@@ -95,6 +95,13 @@ def test_reverse_thread_order_gives_the_same_results(simt_lib):
     run_gpu_tests_emulated(simt_lib, ["tests/test_gpu_reencode.py"], env_extra=rev)
 
 
+def test_edge_streams_emulated_in_both_thread_orders(simt_lib):
+    """tests/test_gpu_edges.py (degenerate shapes, plane-edge windows, extreme coefficients, every wavefront protocol,
+    the lock-step token kernel at 1024 columns) in the default thread order and with SIMT_ORDER=reverse"""
+    run_gpu_tests_emulated(simt_lib, ["tests/test_gpu_edges.py"])
+    run_gpu_tests_emulated(simt_lib, ["tests/test_gpu_edges.py"], env_extra={"SIMT_ORDER": "reverse"})
+
+
 def test_no_misaligned_vector_access_in_the_kernels(simt_lib):
     """x86 tolerates a misaligned uint4 / uint2 / uint32 access, the GPU faults on it: the emulated build once more
     under -fsanitize=alignment (tests/simt/build.sh, SIMT_SANITIZE), over the re-encoding path (the kernels without a
