@@ -10,6 +10,7 @@
 #include <sys/syscall.h>
 #include <unistd.h>
 
+#include <algorithm>
 #include <atomic>
 #include <condition_variable>
 #include <deque>
@@ -982,6 +983,7 @@ class IvfDecode {
   int n_gops = 0;
   // the plan
   int tok_slots = 0, tok_chunk = 1, n_disp = 1, worker_nice = 5;
+  size_t arena_tokens = 0;  // per worker (device-side token decoding)
   bool device_tokens = false;
   // shared between workers and dispatchers
   std::mutex mu;
@@ -1074,13 +1076,24 @@ void IvfDecode::plan() {
     size_t free_mem = 0, total_mem = (size_t)80 << 30;
     if (cudaSetDevice(e->device()) != cudaSuccess || cudaMemGetInfo(&free_mem, &total_mem) != cudaSuccess) total_mem = (size_t)80 << 30;
     const size_t ring_budget = total_mem / 2;
-    const size_t stride = e->token_ring_layout(ring_bytes_for(max_frame_bytes)).stride;
-    int want = (int)(ring_budget / (stride * (size_t)threads));
-    if (want > kTokSlots) want = kTokSlots;
+    // The slots hold records and partitions; the tokens go to an arena per worker, where a frame takes what its own
+    // partitions can produce (Engine::token_cap_for), so that a slot costs what a typical frame needs and not what
+    // the largest one does.  The arena holds at least the largest chunk (half the slots) of the largest frames and
+    // two frames more (a chunk never waits for its own space, and wrapping around wastes less than a frame), and at
+    // most what slots of the largest frame's size would take.
+    const size_t worst = e->token_cap_for(max_frame_bytes), worst_bytes = worst * sizeof(vp8gpu_token);
+    const size_t stride = e->token_ring_layout(ring_bytes_for(max_frame_bytes), true).stride;
+    const size_t per_worker = ring_budget / (size_t)threads;
+    // s * stride + (s / 2 + 2) * worst_bytes <= per_worker
+    int want = per_worker > 2 * worst_bytes ? (int)std::min<size_t>((per_worker - 2 * worst_bytes) / (stride + worst_bytes / 2), kTokSlots) : 0;
     if (knobs.tok_slots >= 0) want = knobs.tok_slots;
     if (want > kTokSlots) want = kTokSlots;
     if (tok_slots > want) tok_slots = want;
     if (tok_slots < 4) tok_slots = 0;  // pool too small: the host workers parse everything
+    if (tok_slots > 0) {
+      const size_t room = per_worker > (size_t)tok_slots * stride ? (per_worker - (size_t)tok_slots * stride) / sizeof(vp8gpu_token) : 0;
+      arena_tokens = std::max(std::min(room, (size_t)tok_slots * worst), (size_t)(tok_slots / 2 + 2) * worst);
+    }
   }
   device_tokens = tok_slots > 0;
   if (!device_tokens) {
@@ -1238,7 +1251,8 @@ ivf_worker_kit* IvfDecode::acquire_kit() {
   {
     std::lock_guard<std::mutex> lk(ctx->pool_mu);
     for (size_t i = 0; i < ctx->kit_pool.size(); i++)
-      if (ctx->kit_pool[i]->ring->bits_cap >= max_frame_bytes + 16 && ctx->kit_pool[i]->ring->nslots >= tok_slots) {
+      if (ctx->kit_pool[i]->ring->bits_cap >= max_frame_bytes + 16 && ctx->kit_pool[i]->ring->nslots >= tok_slots &&
+          ctx->kit_pool[i]->ring->arena_cap >= arena_tokens) {
         k = ctx->kit_pool[i];
         ctx->kit_pool.erase(ctx->kit_pool.begin() + i);
         break;
@@ -1246,7 +1260,7 @@ ivf_worker_kit* IvfDecode::acquire_kit() {
   }
   if (k) return k;
   k = new ivf_worker_kit();
-  bool ok = e->token_ring_create(tok_slots, ring_bytes_for(max_frame_bytes), &k->ring) == VP8GPU_OK &&
+  bool ok = e->token_ring_create(tok_slots, ring_bytes_for(max_frame_bytes), &k->ring, arena_tokens) == VP8GPU_OK &&
             cudaStreamCreateWithFlags(&k->copy_stream, cudaStreamNonBlocking) == cudaSuccess;
   for (cudaStream_t& st : k->kstream) ok = ok && cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking) == cudaSuccess;
   if (!ok) {
@@ -1280,6 +1294,53 @@ void IvfDecode::worker_device(int tid) {
   int rc = VP8GPU_OK;
   ivf_worker_kit* kit = acquire_kit();
   if (!kit) rc = e->fail(VP8GPU_ERR_NOMEM, "decode_ivf: token ring allocation failed");
+  // The token arena is used as a ring in staging order, which is slot order: the space of the oldest frames comes
+  // back first.  live: slots that hold arena space, oldest first; [start, start + len) their tokens.
+  std::deque<int> live;
+  size_t head = 0, a_start[kTokSlots] = {};
+  bool held[kTokSlots] = {};
+  auto arena_take = [&](int si, size_t need, auto in_chunk, vp8gpu_token** out) {
+    const size_t cap = kit->ring->arena_cap;
+    if (held[si]) {  // the slot's previous frame is done: its space is the oldest
+      live.erase(std::find(live.begin(), live.end(), si));
+      held[si] = false;
+    }
+    for (;;) {
+      size_t at = SIZE_MAX;
+      if (live.empty()) {
+        at = need <= cap ? 0 : SIZE_MAX;
+      } else {
+        const size_t tail = a_start[live.front()];
+        if (head > tail) {  // in use: [tail, head)
+          if (cap - head >= need) at = head;
+          else if (tail >= need) at = 0;
+        } else if (tail - head >= need) {  // in use: [tail, end) and [0, head)
+          at = head;
+        }
+      }
+      if (at != SIZE_MAX) {
+        a_start[si] = at;
+        head = at + need;
+        held[si] = true;
+        live.push_back(si);
+        *out = kit->ring->arena + at;
+        return VP8GPU_OK;
+      }
+      // wait for the oldest frame's pixel kernels (plan() sizes the arena so that it is never one of this chunk)
+      if (live.empty() || in_chunk(live.front())) return e->fail(VP8GPU_ERR_LOGIC, "decode_ivf: token arena too small");
+      const int s = live.front();
+      {
+        std::unique_lock<std::mutex> lk(mu);
+        cv_worker[tid].wait(lk, [&] { return slot_state[s] == kFree; });
+      }
+      if (kit->busy[s]) {
+        if (kit->finished[s]) cudaEventSynchronize(kit->finished[s]);
+        kit->busy[s] = false;
+      }
+      live.pop_front();
+      held[s] = false;
+    }
+  };
   while (rc == VP8GPU_OK) {
     const int g = next_gop.fetch_add(1);
     if (g >= n_gops || first_error.load() != VP8GPU_OK) break;
@@ -1312,7 +1373,12 @@ void IvfDecode::worker_device(int tid) {
                                : vp8::parse_frame(state, items[i + c].p, items[i + c].n, p->f, true);
         if (rc != VP8GPU_OK) break;
         count_mbs(p);
-        rc = e->token_ring_stage(kit->ring, si, p->f, kit->copy_stream);
+        vp8gpu_token* tokens = nullptr;
+        rc = arena_take(si, e->token_cap_for(p->f.tw.bits_len), [&](int s) {  // staged in this chunk
+          return (s - first_slot + tok_slots) % tok_slots < c;
+        }, &tokens);
+        if (rc != VP8GPU_OK) break;
+        rc = e->token_ring_stage(kit->ring, si, p->f, kit->copy_stream, tokens);
         if (rc != VP8GPU_OK) break;
         staged++;
         t_slot += t1 - t0;

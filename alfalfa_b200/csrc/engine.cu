@@ -570,16 +570,20 @@ int Engine::build_and_launch(int lane, const DevJob* d_jobs, int* d_sync, int n,
 // ------------------------------------------------------------------------------------------
 // device-side token decoding (tokens.cu)
 // ------------------------------------------------------------------------------------------
-TokenRing Engine::token_ring_layout(size_t max_frame_bytes) const {
+uint32_t Engine::token_cap_for(size_t bits) const {
+  // Every non-zero token ends with a sign decoded at probability 128, which consumes >= 0.98 bit
+  // of the partition, and past the end of the data every block ends at once (only zero bits
+  // arrive): tokens <= 8.2 * bytes + lookahead.  Never more than 25 * 16 per macroblock.
+  const size_t by_bytes = align_up(bits + 16, 256) * 9 + 1024, by_blocks = (size_t)g_.mb_cols * g_.mb_rows * 400;
+  return (uint32_t)(by_bytes < by_blocks ? by_bytes : by_blocks);
+}
+
+TokenRing Engine::token_ring_layout(size_t max_frame_bytes, bool arena) const {
   const size_t n_mbs = (size_t)g_.mb_cols * g_.mb_rows;
   TokenRing r;
   r.bits_cap = (uint32_t)align_up(max_frame_bytes + 16, 256);
   r.split_cap = (uint32_t)n_mbs;
-  // Every non-zero token ends with a sign decoded at probability 128, which consumes >= 0.98 bit
-  // of the partition, and past the end of the data every block ends at once (only zero bits
-  // arrive): tokens <= 8.2 * bytes + lookahead.  Never more than 25 * 16 per macroblock.
-  const size_t by_bytes = (size_t)r.bits_cap * 9 + 1024, by_blocks = n_mbs * 400;
-  r.tok_cap = (uint32_t)(by_bytes < by_blocks ? by_bytes : by_blocks);
+  r.tok_cap = token_cap_for(max_frame_bytes);
   size_t off = 256;  // TokJob
   r.probs_off = off;
   off += 1280;
@@ -597,16 +601,19 @@ TokenRing Engine::token_ring_layout(size_t max_frame_bytes) const {
   r.split_off = off;
   off = align_up(off + (size_t)r.split_cap * sizeof(vp8gpu_split_mvs), 256);
   r.tok_off = off;
-  off = align_up(off + (size_t)r.tok_cap * sizeof(vp8gpu_token), 256);
+  if (!arena) off = align_up(off + (size_t)r.tok_cap * sizeof(vp8gpu_token), 256);
   r.stride = off;
   return r;
 }
 
-int Engine::token_ring_create(int nslots, size_t max_frame_bytes, TokenRing** out) {
+int Engine::token_ring_create(int nslots, size_t max_frame_bytes, TokenRing** out, size_t arena_tokens) {
   CU(cudaSetDevice(device_));
-  TokenRing* r = new TokenRing(token_ring_layout(max_frame_bytes));
+  TokenRing* r = new TokenRing(token_ring_layout(max_frame_bytes, arena_tokens > 0));
   r->nslots = nslots;
+  r->slot_tokens.assign(nslots, nullptr);
+  r->arena_cap = arena_tokens;
   if (cudaMalloc(&r->dev, r->stride * nslots) != cudaSuccess ||
+      (arena_tokens && cudaMalloc(&r->arena, arena_tokens * sizeof(vp8gpu_token)) != cudaSuccess) ||
       cudaHostAlloc(&r->host, r->host_stride * nslots, cudaHostAllocDefault) != cudaSuccess) {
     token_ring_free(r);
     return fail(VP8GPU_ERR_NOMEM, "token ring allocation failed");
@@ -621,20 +628,23 @@ void Engine::token_ring_free(TokenRing* r) {
   if (!r) return;
   cudaSetDevice(device_);
   if (r->dev) cudaFree(r->dev);
+  if (r->arena) cudaFree(r->arena);
   if (r->host) cudaFreeHost(r->host);
   delete r;
 }
 
-int Engine::token_ring_stage(TokenRing* r, int slot, const ParsedFrame& f, cudaStream_t s) {
+int Engine::token_ring_stage(TokenRing* r, int slot, const ParsedFrame& f, cudaStream_t s, vp8gpu_token* tokens) {
   const TokenWork& tw = f.tw;
   if (!tw.deferred) return fail(VP8GPU_ERR_LOGIC, "token_ring_stage: frame was not parsed with defer_tokens");
   if (tw.bits_len > r->bits_cap || f.desc.n_split > r->split_cap)
     return fail(VP8GPU_ERR_NOMEM, "token_ring_stage: frame larger than the ring was sized for");
+  if ((r->arena != nullptr) != (tokens != nullptr)) return fail(VP8GPU_ERR_LOGIC, "token_ring_stage: token area");
   uint8_t* h = r->host_slot(slot);
   uint8_t* d = r->dev_slot(slot);
   TokJob* j = reinterpret_cast<TokJob*>(h);
   j->mbs = reinterpret_cast<vp8gpu_mb*>(d + r->mbs_off);
-  j->tokens = reinterpret_cast<vp8gpu_token*>(d + r->tok_off);
+  j->tokens = tokens ? tokens : reinterpret_cast<vp8gpu_token*>(d + r->tok_off);
+  r->slot_tokens[slot] = j->tokens;
   j->bits = d + r->bits_off;
   j->coef_probs = d + r->probs_off;
   j->result = reinterpret_cast<uint32_t*>(d + r->result_off);
@@ -643,7 +653,7 @@ int Engine::token_ring_stage(TokenRing* r, int slot, const ParsedFrame& f, cudaS
   memcpy(j->part_off, tw.part_off, sizeof(j->part_off));
   memcpy(j->part_len, tw.part_len, sizeof(j->part_len));
   j->nparts = tw.nparts;
-  j->tok_cap = r->tok_cap;
+  j->tok_cap = tokens ? token_cap_for(tw.bits_len) : r->tok_cap;
   memcpy(h + r->probs_off, tw.coef_probs, 1056);
   memcpy(h + r->bits_off, tw.bits, tw.bits_len);
   const size_t n_mbs = (size_t)g_.mb_cols * g_.mb_rows;
@@ -719,7 +729,7 @@ int Engine::submit(int lane, const HostJob* jobs, int n, cudaEvent_t consumed, c
       if (j.ring) {
         const uint8_t* slot = j.ring->dev_slot(j.ring_slot);
         d.mbs = reinterpret_cast<const vp8gpu_mb*>(slot + j.ring->mbs_off);
-        d.tokens = reinterpret_cast<const vp8gpu_token*>(slot + j.ring->tok_off);
+        d.tokens = j.ring->slot_tokens[j.ring_slot];
         d.split = reinterpret_cast<const vp8gpu_split_mvs*>(slot + j.ring->split_off);
       } else {
         d.mbs = reinterpret_cast<const vp8gpu_mb*>(st.dev + L.mbs_off[i]);

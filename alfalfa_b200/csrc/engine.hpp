@@ -19,14 +19,19 @@ constexpr int kStagingDepth = 3;    // device record buffers in flight per lane
 
 // Device + pinned staging for frames whose DCT partitions are decoded on the device (tokens.cu):
 // `nslots` slots of equal size in one allocation, so that consecutive slots can share one launch.
-// Device slot: TokJob | probabilities | partitions | result words | mbs | split MVs | tokens.
+// Device slot: TokJob | probabilities | partitions | result words | mbs | split MVs | tokens.  A ring created with a
+// token arena has no token part in its slots: the caller hands every staged frame a piece of the arena sized for that
+// frame's partitions (token_cap_for), so the slots cost what a typical frame needs, not what the largest one does.
 struct TokenRing {
   int nslots = 0;
   uint8_t* dev = nullptr;
   uint8_t* host = nullptr;       // pinned mirror of the first three parts of every slot
   size_t stride = 0, host_stride = 0;
   size_t probs_off = 0, info_off = 0, bits_off = 0, result_off = 0, above_off = 0, mbs_off = 0, split_off = 0, tok_off = 0;
-  uint32_t bits_cap = 0, split_cap = 0, tok_cap = 0;
+  uint32_t bits_cap = 0, split_cap = 0, tok_cap = 0;  // tok_cap: tokens of a frame of bits_cap partition bytes
+  vp8gpu_token* arena = nullptr;  // tokens of the slots when not in the slots themselves
+  size_t arena_cap = 0;           // in tokens
+  std::vector<vp8gpu_token*> slot_tokens;  // where the tokens of each slot's current frame go
   uint8_t* dev_slot(int i) const { return dev + (size_t)i * stride; }
   uint8_t* host_slot(int i) const { return host + (size_t)i * host_stride; }
 };
@@ -98,11 +103,16 @@ class Engine {
   int submit(int lane, const HostJob* jobs, int n, cudaEvent_t consumed, cudaEvent_t* between = nullptr);
 
   // device-side token decoding
-  TokenRing token_ring_layout(size_t max_frame_bytes) const;  // offsets and capacities only
-  int token_ring_create(int nslots, size_t max_frame_bytes, TokenRing** out);
+  // offsets and capacities only; arena: no token part in the slots
+  TokenRing token_ring_layout(size_t max_frame_bytes, bool arena = false) const;
+  // the most tokens k_tokens can write for partitions of `bits` bytes (the capacity rule of token_ring_layout)
+  uint32_t token_cap_for(size_t bits) const;
+  // arena_tokens > 0: the slots' tokens go to a separate arena of that many tokens (see TokenRing)
+  int token_ring_create(int nslots, size_t max_frame_bytes, TokenRing** out, size_t arena_tokens = 0);
   void token_ring_free(TokenRing* r);
-  // queue on `s` the upload of one frame parsed with defer_tokens (records + partitions)
-  int token_ring_stage(TokenRing* r, int slot, const ParsedFrame& f, cudaStream_t s);
+  // queue on `s` the upload of one frame parsed with defer_tokens (records + partitions); a ring with an arena
+  // takes the frame's token area (`tokens`, token_cap_for(f.tw.bits_len) tokens) from the caller
+  int token_ring_stage(TokenRing* r, int slot, const ParsedFrame& f, cudaStream_t s, vp8gpu_token* tokens = nullptr);
   // one k_tokens launch over `count` consecutive slots (wrapping around the ring)
   int token_ring_launch(TokenRing* r, int first, int count, cudaStream_t s);
   // synchronous: tokens written / overflow flag of a slot whose kernel has been queued on `s`
