@@ -455,6 +455,7 @@ int vp8gpu_parse_frame_device(vp8gpu_ctx* ctx, vp8gpu_state* state, const uint8_
   if (rc != VP8GPU_OK) return rc;
   cudaStream_t s = e->stream(0);
   rc = e->token_ring_stage(r, 0, out->f, s);
+  if (rc == VP8GPU_OK) rc = e->token_ring_clear_result(r, 0, s);
   if (rc == VP8GPU_OK) rc = e->token_ring_launch(r, 0, 1, s);
   uint32_t result[2] = {0, 0};
   if (rc == VP8GPU_OK) rc = e->token_ring_result(r, 0, s, result);
@@ -918,9 +919,10 @@ struct IvfKnobs {
   int tok_slots = -1;      // VP8GPU_TOK_SLOTS     frames a worker keeps between "first partition parsed" and "pixels done"
   int tok_chunk = -1;      // VP8GPU_TOK_CHUNK     frames per token-kernel launch
   int tok_inflight = -1;   // VP8GPU_TOK_INFLIGHT  cap on frames inside token kernels (0 = unlimited)
+  int tok_arena = -1;      // VP8GPU_TOK_ARENA     token arena per worker, in largest frames (never below plan()'s floor)
   int dispatchers = -1;    // VP8GPU_DISPATCHERS   dispatcher threads
   int worker_nice = -1;    // VP8GPU_WORKER_NICE   niceness of the parsing workers (0 = leave alone)
-  bool trace = false;      // VP8GPU_TRACE         per-batch device times on stderr
+  bool trace = false;      // VP8GPU_TRACE         per-batch device times and per-worker arena counters on stderr
   bool parse_cache = false;  // VP8GPU_PARSE_CACHE  diagnostic: replay remembered first partitions (see above)
   static int num(const char* name) {
     const char* v = getenv(name);
@@ -928,8 +930,8 @@ struct IvfKnobs {
   }
   IvfKnobs()
       : tok_slots(num("VP8GPU_TOK_SLOTS")), tok_chunk(num("VP8GPU_TOK_CHUNK")), tok_inflight(num("VP8GPU_TOK_INFLIGHT")),
-        dispatchers(num("VP8GPU_DISPATCHERS")), worker_nice(num("VP8GPU_WORKER_NICE")), trace(getenv("VP8GPU_TRACE") != nullptr),
-        parse_cache(getenv("VP8GPU_PARSE_CACHE") != nullptr) {}
+        tok_arena(num("VP8GPU_TOK_ARENA")), dispatchers(num("VP8GPU_DISPATCHERS")), worker_nice(num("VP8GPU_WORKER_NICE")),
+        trace(getenv("VP8GPU_TRACE") != nullptr), parse_cache(getenv("VP8GPU_PARSE_CACHE") != nullptr) {}
 };
 
 // vp8gpu_decode_ivf as an object, one instance per call: parse_container() reads the IVF file into GOPs, plan() sizes
@@ -1093,6 +1095,9 @@ void IvfDecode::plan() {
     if (tok_slots > 0) {
       const size_t room = per_worker > (size_t)tok_slots * stride ? (per_worker - (size_t)tok_slots * stride) / sizeof(vp8gpu_token) : 0;
       arena_tokens = std::max(std::min(room, (size_t)tok_slots * worst), (size_t)(tok_slots / 2 + 2) * worst);
+      // VP8GPU_TOK_ARENA=<n>: room for n largest frames, never less than the floor above, so that a small stream on a large device can run
+      // the allocator in the regime of a memory-bound plan (many workers, large frames)
+      if (knobs.tok_arena >= 0) arena_tokens = std::max((size_t)knobs.tok_arena * worst, (size_t)(tok_slots / 2 + 2) * worst);
     }
   }
   device_tokens = tok_slots > 0;
@@ -1258,7 +1263,7 @@ ivf_worker_kit* IvfDecode::acquire_kit() {
         break;
       }
   }
-  if (k) return k;
+  if (k) return k;  // its overflow flags are clear: worker_device clears a flagged slot before pooling the kit
   k = new ivf_worker_kit();
   bool ok = e->token_ring_create(tok_slots, ring_bytes_for(max_frame_bytes), &k->ring, arena_tokens) == VP8GPU_OK &&
             cudaStreamCreateWithFlags(&k->copy_stream, cudaStreamNonBlocking) == cudaSuccess;
@@ -1296,11 +1301,14 @@ void IvfDecode::worker_device(int tid) {
   if (!kit) rc = e->fail(VP8GPU_ERR_NOMEM, "decode_ivf: token ring allocation failed");
   // The token arena is used as a ring in staging order, which is slot order: the space of the oldest frames comes
   // back first.  live: slots that hold arena space, oldest first; [start, start + len) their tokens.
+  // The plan's size, not the kit's: a kit from an earlier call may hold a larger arena.
+  // Counters (VP8GPU_TRACE): pieces taken, pieces placed back at offset 0, frames waited for to free space.
   std::deque<int> live;
   size_t head = 0, a_start[kTokSlots] = {};
   bool held[kTokSlots] = {};
+  long n_takes = 0, n_wraps = 0, n_waits = 0;
   auto arena_take = [&](int si, size_t need, auto in_chunk, vp8gpu_token** out) {
-    const size_t cap = kit->ring->arena_cap;
+    const size_t cap = arena_tokens;
     if (held[si]) {  // the slot's previous frame is done: its space is the oldest
       live.erase(std::find(live.begin(), live.end(), si));
       held[si] = false;
@@ -1319,6 +1327,8 @@ void IvfDecode::worker_device(int tid) {
         }
       }
       if (at != SIZE_MAX) {
+        n_takes++;
+        if (at == 0 && head > 0) n_wraps++;
         a_start[si] = at;
         head = at + need;
         held[si] = true;
@@ -1329,6 +1339,7 @@ void IvfDecode::worker_device(int tid) {
       // wait for the oldest frame's pixel kernels (plan() sizes the arena so that it is never one of this chunk)
       if (live.empty() || in_chunk(live.front())) return e->fail(VP8GPU_ERR_LOGIC, "decode_ivf: token arena too small");
       const int s = live.front();
+      n_waits++;
       {
         std::unique_lock<std::mutex> lk(mu);
         cv_worker[tid].wait(lk, [&] { return slot_state[s] == kFree; });
@@ -1471,13 +1482,23 @@ void IvfDecode::worker_device(int tid) {
     cudaStreamSynchronize(kit->copy_stream);
     for (cudaStream_t st : kit->kstream) cudaStreamSynchronize(st);
     // k_tokens reports a token pool that was too small instead of writing out of bounds; the capacity
-    // rule (Engine::token_ring_layout) makes that impossible, so a set flag is an internal error
+    // rule (Engine::token_ring_layout) makes that impossible, so a set flag is an internal error.  The flag is
+    // sticky: it covers every frame this call staged in the slot, not only the last one.  A kit goes back to the pool
+    // with every flag clear (slots beyond tok_slots were not used by this call and are still clear).
     uint32_t res[kTokSlots][2];
     if (cudaMemcpy2D(res, 8, kit->ring->dev + kit->ring->result_off, kit->ring->stride, 8, (size_t)kit->ring->nslots,
                      cudaMemcpyDeviceToHost) == cudaSuccess) {
+      bool cleared = false;
       for (int k = 0; k < kit->ring->nslots && k < tok_slots; k++)
-        if (res[k][1]) set_error(e->fail(VP8GPU_ERR_LOGIC, "device token pool overflow"));
+        if (res[k][1]) {
+          set_error(e->fail(VP8GPU_ERR_LOGIC, "device token pool overflow"));
+          cleared = e->token_ring_clear_result(kit->ring, k, kit->copy_stream) == VP8GPU_OK || cleared;
+        }
+      if (cleared) cudaStreamSynchronize(kit->copy_stream);
     }
+    if (knobs.trace)
+      fprintf(stderr, "decode_ivf arena: worker %d takes %ld wraps %ld waits %ld cap %zu slots %d chunk %d\n", tid, n_takes, n_wraps,
+              n_waits, arena_tokens, tok_slots, tok_chunk);
     std::lock_guard<std::mutex> lk(ctx->pool_mu);
     ctx->kit_pool.push_back(kit);
   }

@@ -682,6 +682,11 @@ int Engine::token_ring_launch(TokenRing* r, int first, int count, cudaStream_t s
   return VP8GPU_OK;
 }
 
+int Engine::token_ring_clear_result(TokenRing* r, int slot, cudaStream_t s) {
+  CU(cudaMemsetAsync(r->dev_slot(slot) + r->result_off, 0, 8, s));
+  return VP8GPU_OK;
+}
+
 int Engine::token_ring_result(TokenRing* r, int slot, cudaStream_t s, uint32_t result[2]) {
   CU(cudaMemcpyAsync(result, r->dev_slot(slot) + r->result_off, 8, cudaMemcpyDeviceToHost, s));
   CU(cudaStreamSynchronize(s));

@@ -115,6 +115,9 @@ class Engine {
   int token_ring_stage(TokenRing* r, int slot, const ParsedFrame& f, cudaStream_t s, vp8gpu_token* tokens = nullptr);
   // one k_tokens launch over `count` consecutive slots (wrapping around the ring)
   int token_ring_launch(TokenRing* r, int first, int count, cudaStream_t s);
+  // queue on `s` the reset of a slot's result words; k_tokens only ever sets the overflow flag, so it stays set for
+  // all the frames staged in the slot until this runs (token_ring_create starts every slot clear)
+  int token_ring_clear_result(TokenRing* r, int slot, cudaStream_t s);
   // synchronous: tokens written / overflow flag of a slot whose kernel has been queued on `s`
   int token_ring_result(TokenRing* r, int slot, cudaStream_t s, uint32_t result[2]);
 

@@ -228,7 +228,8 @@ TK_DEV void decode_frame_tokens(const TokJob& J, const Geom& g, const uint8_t* p
     parts[row & (nparts - 1)] = tr;
   }
   J.result[0] = static_cast<uint32_t>(t - t_begin);
-  J.result[1] = overflow;
+  // sticky: a slot's result words serve all the frames staged in it, and the host reads the flag once for all of them
+  if (overflow) J.result[1] = 1;
 }
 
 
@@ -515,7 +516,7 @@ TK_DEV void decode_frame_tokens_lockstep(const TokJob& J, const Geom& g, const L
     }
   }
   J.result[0] = static_cast<uint32_t>(t - t_begin);
-  J.result[1] = overflow;
+  if (overflow) J.result[1] = 1;  // sticky, as in decode_frame_tokens
 }
 
 }  // namespace tok

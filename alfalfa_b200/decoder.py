@@ -383,8 +383,8 @@ def decode_ivf(ctx, ivf_bytes, threads=1, want_output=True):
         check(L.vp8gpu_decode_ivf(ctx.h, ivf_bytes, len(ivf_bytes), threads, ptr, size if ptr else 0, C.byref(nd),
                                   C.byref(ns)), ctx.h, "decode_ivf")
         check(L.vp8gpu_ctx_sync(ctx.h), ctx.h, "sync")
-        if ptr:
-            dst = C.string_at(ptr, ns.value * ctx.display_bytes)
+        if ptr:  # not C.string_at: its length is a C int, and an output of 2 GiB or more came back truncated
+            dst = bytes((C.c_uint8 * (ns.value * ctx.display_bytes)).from_address(ptr.value))
     finally:
         if ptr:
             L.vp8gpu_host_free(ptr)

@@ -102,6 +102,15 @@ def test_edge_streams_emulated_in_both_thread_orders(simt_lib):
     run_gpu_tests_emulated(simt_lib, ["tests/test_gpu_edges.py"], env_extra={"SIMT_ORDER": "reverse"})
 
 
+def test_stream_pipeline_emulated_in_both_thread_orders(simt_lib):
+    """tests/test_gpu_stream_pipeline.py (the densest tokens, the token arena's counters against the allocator model,
+    dispatcher and permit knobs, worker kits reused across calls) in the default thread order and with
+    SIMT_ORDER=reverse; the 1080p and 64-worker cases stay on the GPU"""
+    args = ["tests/test_gpu_stream_pipeline.py", "-k", "not 1920x1080 and not bench"]
+    run_gpu_tests_emulated(simt_lib, args)
+    run_gpu_tests_emulated(simt_lib, args, env_extra={"SIMT_ORDER": "reverse"})
+
+
 def test_no_misaligned_vector_access_in_the_kernels(simt_lib):
     """x86 tolerates a misaligned uint4 / uint2 / uint32 access, the GPU faults on it: the emulated build once more
     under -fsanitize=alignment (tests/simt/build.sh, SIMT_SANITIZE), over the re-encoding path (the kernels without a

@@ -65,10 +65,10 @@ def serialize(L, capi, hdr, ft, mbs, tokens, split):
 
 def ivf(w, h, chunks):
     """-> IVF bytes (util/ivf.cc:36-82)"""
-    out = struct.pack("<4sHH4sHHIII", b"DKIF", 0, 32, b"VP80", w, h, 30, 1, len(chunks)) + b"\0\0\0\0"
+    out = [struct.pack("<4sHH4sHHIII", b"DKIF", 0, 32, b"VP80", w, h, 30, 1, len(chunks)) + b"\0\0\0\0"]
     for i, c in enumerate(chunks):
-        out += struct.pack("<IQ", len(c), i) + c
-    return out
+        out += [struct.pack("<IQ", len(c), i), c]
+    return b"".join(out)   # joined once: the tests build streams of thousands of frames
 
 
 def make_frame(rng, L, capi, w, h, index, saved_probs, all_bpred=False):
