@@ -5,7 +5,8 @@ own under a timeout: a hang or a CUDA fault fails that one test and nothing else
 usage: python reencode_worker.py IN.pickle OUT.pickle     |     python reencode_worker.py errors
   IN:  dict(w, h, targets=[(y, u, v) ...], pred=[bytes ...], state=bytes, kf_q_weight, extra_frame_chunk)
   OUT: dict(frames=[bytes ...], in_step=bool)   in_step: a Decoder resumed from `state` that decodes the emitted frames
-                                                equals Encoder::export_decoder() at the end"""
+                                                equals Encoder::export_decoder() at the end
+  IN a list of such dicts: OUT the list of their results, dict(error=str) where the library refused the case"""
 import os
 import pickle
 import sys
@@ -14,8 +15,22 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
 
 def main():
-    from alfalfa_b200 import Context, Decoder, Encoder
     a = pickle.load(open(sys.argv[1], "rb"))
+    if isinstance(a, list):   # several cases: an error of the library is reported per case instead of ending the run
+        from alfalfa_b200 import capi
+        out = []
+        for case in a:
+            try:
+                out.append(run(case))
+            except (capi.Invalid, capi.Unsupported, capi.LogicError) as e:
+                out.append({"error": "%s: %s" % (type(e).__name__, e)})
+    else:
+        out = run(a)
+    pickle.dump(out, open(sys.argv[2], "wb"))
+
+
+def run(a):
+    from alfalfa_b200 import Context, Decoder, Encoder
     w, h = a["w"], a["h"]
     ctx = Context(w, h, max_frames=24)
     pred_decoder = Decoder(ctx)  # the prediction stream's own decoder (xc-enc.cc:254, 284-300)
@@ -30,8 +45,9 @@ def main():
     for c in frames:
         rx.get_frame_output(c)
     in_step = rx == enc.export_decoder()
-    pickle.dump({"frames": frames, "in_step": bool(in_step)}, open(sys.argv[2], "wb"))
+    del enc, rx, pred_decoder
     ctx.close()
+    return {"frames": frames, "in_step": bool(in_step)}
 
 
 def errors():

@@ -78,17 +78,32 @@ def make_case(w, h, n, qi_a, qi_b):
 def product_reencode(w, h, targets, pred_chunks, state_blob, kf_q_weight, extra_frame_chunk, timeout=300, env=None):
     """the product's Encoder::reencode in a child process (tests/reencode_worker.py) under a timeout: returns
     (emitted frames, receiver-in-step flag)"""
+    out = _run_worker(_case(w, h, targets, pred_chunks, state_blob, kf_q_weight, extra_frame_chunk), timeout, env)
+    return out["frames"], out["in_step"]
+
+
+def product_reencode_cases(cases, timeout=300):
+    """product_reencode of several cases, each a tuple of its first seven arguments, in one child process: per case
+    (emitted frames, in-step flag), or the error message where the library refused it"""
+    out = _run_worker([_case(*c) for c in cases], timeout)
+    return [o["error"] if "error" in o else (o["frames"], o["in_step"]) for o in out]
+
+
+def _case(w, h, targets, pred_chunks, state_blob, kf_q_weight, extra_frame_chunk):
+    return dict(w=w, h=h, targets=[tuple(np.ascontiguousarray(p) for p in t) for t in targets], pred=list(pred_chunks),
+                state=bytes(state_blob), kf_q_weight=kf_q_weight, extra_frame_chunk=bool(extra_frame_chunk))
+
+
+def _run_worker(job, timeout, env=None):
     import pickle
     import sys
     with tempfile.TemporaryDirectory() as d:
         fin, fout = os.path.join(d, "in.pickle"), os.path.join(d, "out.pickle")
-        pickle.dump(dict(w=w, h=h, targets=[tuple(np.ascontiguousarray(p) for p in t) for t in targets], pred=list(pred_chunks),
-                         state=bytes(state_blob), kf_q_weight=kf_q_weight, extra_frame_chunk=bool(extra_frame_chunk)), open(fin, "wb"))
+        pickle.dump(job, open(fin, "wb"))
         r = subprocess.run([sys.executable, os.path.join(ROOT, "tests", "reencode_worker.py"), fin, fout], capture_output=True, text=True,
                            timeout=timeout, env=dict(os.environ, **(env or {})))
         assert r.returncode == 0, (r.stdout + r.stderr)[-1500:]
-        out = pickle.load(open(fout, "rb"))
-    return out["frames"], out["in_step"]
+        return pickle.load(open(fout, "rb"))
 
 
 def test_whole_chunk_the_same_with_the_shortcuts_off():

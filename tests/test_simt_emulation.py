@@ -102,6 +102,13 @@ def test_edge_streams_emulated_in_both_thread_orders(simt_lib):
     run_gpu_tests_emulated(simt_lib, ["tests/test_gpu_edges.py"], env_extra={"SIMT_ORDER": "reverse"})
 
 
+def test_reencode_edges_emulated_in_both_thread_orders(simt_lib):
+    """tests/test_gpu_reencode_edges.py (re-encoding at degenerate shapes, plane-edge windows and saturated targets)
+    in the default thread order and with SIMT_ORDER=reverse; the 1080p and 16383-pixel-wide cases stay on the GPU"""
+    run_gpu_tests_emulated(simt_lib, ["tests/test_gpu_reencode_edges.py"])
+    run_gpu_tests_emulated(simt_lib, ["tests/test_gpu_reencode_edges.py"], env_extra={"SIMT_ORDER": "reverse"})
+
+
 def test_stream_pipeline_emulated_in_both_thread_orders(simt_lib):
     """tests/test_gpu_stream_pipeline.py (the densest tokens, the token arena's counters against the allocator model,
     dispatcher and permit knobs, worker kits reused across calls) in the default thread order and with

@@ -20,6 +20,10 @@ starts 2 pixels before and is 9 wide.  In mv_edges only macroblocks at even rows
 the others are intra-coded or ZEROMV, so the writer's vector prediction is 0 and every vector up to +-2046
 eighth-pels can be coded as it was chosen.
 
+Each family can also be written without segmentation (segment_maps=False), the form in which
+Encoder::update_residues takes it (a prediction frame that updates the segment map is refused, and with segments the
+reference's encoder drifts from its receiver, DESIGN.md section 5): make_reencodable() / reencode_names().
+
 usage: python tools/make_edge_stream.py NAME OUT.ivf        (NAME one of names())
 """
 import os
@@ -170,8 +174,8 @@ def _sparse_tokens(rng, m, tokens):
 
 
 # ---------------------------------------------------------------- shapes
-def make_shape(w, h, all_bpred, seed):
-    return F.make_stream(w, h, SHAPE_FRAMES, seed, all_bpred=all_bpred)
+def make_shape(w, h, all_bpred, seed, segment_maps=True, frames=SHAPE_FRAMES):
+    return F.make_stream(w, h, frames, seed, all_bpred=all_bpred, segment_maps=segment_maps)
 
 
 # ---------------------------------------------------------------- mv_edges
@@ -211,15 +215,16 @@ def _luma_subs(c, k):
     return subs
 
 
-def make_mv_edges(w, h, frames, seed):
-    """-> (IVF bytes, intended): intended[i] = {macroblock index: (16, 2) vectors} of every aimed macroblock of frame i"""
+def make_mv_edges(w, h, frames, seed, segment_maps=True):
+    """-> (IVF bytes, intended): intended[i] = {macroblock index: (16, 2) vectors} of every aimed macroblock of frame i.
+    segment_maps=False: the key frame without segmentation (the inter frames never use it)"""
     L, capi = _lib()
     rng = np.random.default_rng(seed)
     saved = np.zeros(1056, dtype=np.uint8)
     cols, rows = (w + 15) // 16, (h + 15) // 16
     PY, PC = (16 * cols, 16 * rows), (8 * cols, 8 * rows)
     sched = {(path, plane, axis): _Schedule(plane) for path in ("16x16", "split") for plane in "YC" for axis in "xy"}
-    chunks, intended = [F.make_frame(rng, L, capi, w, h, 0, saved)], [{}]
+    chunks, intended = [F.make_frame(rng, L, capi, w, h, 0, saved, segment_maps=segment_maps)], [{}]
     refs = [REF_LAST, REF_GOLDEN, REF_ALTREF]
     kinds = ["c16", "y16", "csplit", "c16", "ysplit", "csplit", "y16"]   # 7: every kind reaches every grid position
     nk = nref = nround = 0
@@ -297,7 +302,8 @@ COEFF_FRAMES = [(127, +1, (0, 127, 28, 57)), (0, -1, (0, 127, 28, 57)), (127, +1
 ZERO_TOKEN = {28: 2048, 57: 1024}   # y_ac 32 / 64
 
 
-def make_coeffs(w, h, seed):
+def make_coeffs(w, h, seed, segment_maps=True):
+    """segment_maps=False: no segmentation (so no segment-map update in the inter frames)"""
     L, capi = _lib()
     rng = np.random.default_rng(seed)
     saved = np.zeros(1056, dtype=np.uint8)
@@ -317,6 +323,8 @@ def make_coeffs(w, h, seed):
         for name in ("y_dc_delta", "y2_dc_delta", "y2_ac_delta", "uv_dc_delta", "uv_ac_delta"):
             setattr(ft, name, 15 * sign)
         ft.segmentation_enabled = ft.update_mb_segmentation_map = ft.update_segment_feature_data = 1
+        if not segment_maps:
+            ft.segmentation_enabled = ft.update_mb_segmentation_map = ft.update_segment_feature_data = 0
         ft.segment_feature_absolute = int(seg_abs is not None)
         for i in range(4):
             ft.segment_quant[i] = seg_abs[i] if seg_abs else (-127, 127, -15, 15)[i]
@@ -407,9 +415,85 @@ def make(name):
     raise KeyError(name)
 
 
-if __name__ == "__main__":
-    if len(sys.argv) != 3:
-        sys.exit(__doc__ + "\nnames: " + " ".join(names()))
-    data = make(sys.argv[1])
-    open(sys.argv[2], "wb").write(data)
-    print("%s: %d bytes" % (sys.argv[2], len(data)))
+# ---------------------------------------------------------------- re-encoding
+# Prediction streams for Encoder::update_residues / reencode_as_interframe: the families above written with
+# segment_maps=False.
+# (width, height): 1 MB, 1 column, 1 row (128 columns: four words of k_reenc_intra's intra bitmask), 2 and 3 columns
+# (the wavefront's lag is clamped at the last column), an MB-aligned width of 16 mod 32 (row pitch > width), 1024
+# columns (the bitmask's limit), each also at an odd display size.  Every intra macroblock uses B_PRED (the
+# above-right edge and the lag only matter there; the other families carry the 16 x 16 modes), and 12 frames give
+# intra macroblocks of inter frames in the first and the last column of every shape.
+REENCODE_SHAPES = [(1, 1), (16, 16), (17, 17), (16, 512), (15, 511), (2048, 16), (2047, 15), (32, 64), (31, 63), (48, 64),
+                   (47, 63), (208, 64), (207, 63), (16383, 32), (16383, 17)]
+REENCODE_SHAPE_FRAMES = 12
+SATURATE_SIZES = [(64, 48), (47, 33)]
+SATURATE_FRAMES = 10
+PREVIOUS_SEED = 1000   # the previous chunk: the same family at the same size, another seed
+
+
+# ---------------------------------------------------------------- saturate
+def make_saturate(w, h, seed, tokens):
+    """q index 0 frames without deltas, loop filter off, one partition.  The key frame is DC_PRED throughout; in
+    every inter frame macroblock 0 is DC_PRED (its predictor is flat: 128 in all planes, whatever came before), the
+    others cycle through ZEROMV from LAST (with Y2), SPLITMV with zero vectors from LAST, B_PRED and ZEROMV again, and
+    LAST is refreshed: a target against which every residue is +-255 or dense is a target that flips against the
+    previous frame.  tokens=False: no coefficients at all, so that what a receiver decodes is exactly the prediction
+    of every macroblock (the zero-residue targets); tokens=True: sparse coefficients (a picture that is not flat, for
+    the previous chunk)."""
+    L, capi = _lib()
+    rng = np.random.default_rng(seed)
+    saved = np.zeros(1056, dtype=np.uint8)
+    cols, rows = (w + 15) // 16, (h + 15) // 16
+    chunks = []
+    for index in range(SATURATE_FRAMES):
+        key = index == 0
+        hdr = _header(capi, w, h, key, True, 0, 0, 0)
+        ft = capi.EncodeFeatures()
+        ft.refresh_last = 1
+        ft.refresh_entropy_probs = 1
+        ft.saved_coef_probs = saved.ctypes.data
+        mbs = np.zeros(cols * rows, dtype=capi.MB_DTYPE)
+        split, toks = [], []
+        for i in range(cols * rows):
+            m = mbs[i]
+            kind = 0 if key or i == 0 else 1 + (i + index) % 4
+            if kind == 0:
+                m["ref_frame"], m["y_mode"], m["uv_mode"] = REF_CURRENT, DC_PRED, DC_PRED
+            elif kind == 3:
+                m["ref_frame"], m["y_mode"] = REF_CURRENT, B_PRED
+                m["uv_mode"] = int(rng.integers(0, 4))
+                m["b_modes"] = int(sum(int(rng.integers(0, 10)) << (4 * k) for k in range(16)))
+            else:
+                m["ref_frame"], m["y_mode"] = REF_LAST, ZEROMV
+                if kind == 2:
+                    m["y_mode"], m["split_idx"] = SPLITMV, len(split)
+                    split.append(np.zeros((16, 2), dtype=np.int16))
+            if tokens:
+                _sparse_tokens(rng, m, toks)
+            else:
+                m["flags"] = 1 if m["y_mode"] not in (B_PRED, SPLITMV) else 0
+        chunks.append(F.serialize(L, capi, hdr, ft, mbs, toks, split))
+    return F.ivf(w, h, chunks)
+
+
+def reencode_names():
+    return (["shapes_%dx%d" % s for s in REENCODE_SHAPES] + ["mv_edges_%dx%d" % s for s in MV_EDGE_SIZES] +
+            ["coeffs_%dx%d" % s for s in COEFF_SIZES] + ["saturate_%dx%d" % s for s in SATURATE_SIZES])
+
+
+def make_reencodable(name, previous=False):
+    """IVF bytes of the re-encoding prediction stream `name` (one of reencode_names()); previous: the stream whose
+    state the re-encoded chunk starts from"""
+    family, size = name.rsplit("_", 1)
+    w, h = (int(x) for x in size.split("x"))
+    seed = PREVIOUS_SEED if previous else 0
+    if family == "shapes":
+        k = REENCODE_SHAPES.index((w, h))
+        return make_shape(w, h, True, 600 + k + seed, segment_maps=False, frames=REENCODE_SHAPE_FRAMES)
+    if family == "mv_edges":
+        return make_mv_edges(w, h, MV_EDGE_FRAMES, 400 + w + seed, segment_maps=False)[0]
+    if family == "coeffs":
+        return make_coeffs(w, h, 500 + w + seed, segment_maps=False)
+    if family == "saturate":
+        return make_saturate(w, h, 800 + w + seed, tokens=previous)
+    raise KeyError(name)

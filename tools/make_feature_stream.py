@@ -71,8 +71,9 @@ def ivf(w, h, chunks):
     return b"".join(out)   # joined once: the tests build streams of thousands of frames
 
 
-def make_frame(rng, L, capi, w, h, index, saved_probs, all_bpred=False):
-    """all_bpred: every intra macroblock uses B_PRED (the draws are the same either way)"""
+def make_frame(rng, L, capi, w, h, index, saved_probs, all_bpred=False, segment_maps=True):
+    """all_bpred: every intra macroblock uses B_PRED; segment_maps=False: no segmentation (so no segment-map
+    update in inter frames, the form re-encoding takes) (the draws are the same either way)"""
     cols, rows = (w + 15) // 16, (h + 15) // 16
     n = cols * rows
     key = index == 0
@@ -107,6 +108,8 @@ def make_frame(rng, L, capi, w, h, index, saved_probs, all_bpred=False):
                 ft.segment_lf[i] = int(rng.integers(-63, 64))
         for i in range(3):
             ft.segment_tree_probs[i] = int(rng.integers(1, 255)) if rng.random() < 0.8 else 255
+        if not segment_maps:
+            ft.segmentation_enabled = ft.update_mb_segmentation_map = ft.update_segment_feature_data = 0
     if rng.random() < 0.6:
         ft.lf_delta_enabled = 1
         ft.lf_delta_update = int(rng.random() < 0.7)
@@ -181,13 +184,13 @@ def make_frame(rng, L, capi, w, h, index, saved_probs, all_bpred=False):
     return serialize(L, capi, hdr, ft, mbs, tokens, split)
 
 
-def make_stream(w, h, frames, seed, all_bpred=False):
+def make_stream(w, h, frames, seed, all_bpred=False, segment_maps=True):
     """-> IVF bytes"""
     from alfalfa_b200 import capi
     L = capi.lib()
     rng = np.random.default_rng(seed)
     saved = np.zeros(1056, dtype=np.uint8)
-    return ivf(w, h, [make_frame(rng, L, capi, w, h, i, saved, all_bpred) for i in range(frames)])
+    return ivf(w, h, [make_frame(rng, L, capi, w, h, i, saved, all_bpred, segment_maps) for i in range(frames)])
 
 
 if __name__ == "__main__":

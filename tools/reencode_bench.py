@@ -19,29 +19,29 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
 
-def main():
-    ap = argparse.ArgumentParser()
-    ap.add_argument("--frames", type=int, default=12)
-    ap.add_argument("--device", type=int, default=0)
-    ap.add_argument("--prev", default=os.path.join(ROOT, "bench_data", "synth1080p_easy_q40.ivf"))
-    ap.add_argument("--chunk", default=os.path.join(ROOT, "bench_data", "synth1080p_medium_q90.ivf"))
-    ap.add_argument("--kf-q-weight", type=float, default=0.75)
-    a = ap.parse_args()
+PREV = os.path.join(ROOT, "bench_data", "synth1080p_easy_q40.ivf")
+CHUNK = os.path.join(ROOT, "bench_data", "synth1080p_medium_q90.ivf")
+PREV_FRAMES = 8
+
+
+def bench_inputs(ctx, prev_path=PREV, chunk_path=CHUNK, frames=12):
+    """The inputs of the measured re-encode: the state PREV_FRAMES frames of `prev_path` leave behind (Decoder::
+    serialize, the reference's own format, tests/test_state_format.py), the first `frames` frames of `chunk_path`,
+    parsed with keep_labels by their own decoder, and their decoded pictures as targets.  ctx: a Context of the
+    clips' size.  -> (state, chunk, prediction_frames, targets)"""
     import numpy as np
 
-    from alfalfa_b200 import Context, Decoder, Encoder
-    from alfalfa_b200.decoder import read_ivf, write_ivf
+    from alfalfa_b200 import Decoder
+    from alfalfa_b200.decoder import read_ivf
 
-    w, h, prev = read_ivf(open(a.prev, "rb").read())
-    w2, h2, chunk = read_ivf(open(a.chunk, "rb").read())
-    assert (w, h) == (w2, h2)
-    chunk = chunk[:a.frames]
-    prev = prev[:8]
-    ctx = Context(w, h, device=a.device, max_frames=32)
+    w, h, prev = read_ivf(open(prev_path, "rb").read())
+    w2, h2, chunk = read_ivf(open(chunk_path, "rb").read())
+    assert (w, h) == (w2, h2) == (ctx.width, ctx.height)
+    chunk = chunk[:frames]
     d = Decoder(ctx)
-    for c in prev:
+    for c in prev[:PREV_FRAMES]:
         d.get_frame_output(c)
-    state = d.serialize()  # Decoder::serialize, the reference's own format (tests/test_state_format.py)
+    state = d.serialize()
     pred_decoder = Decoder(ctx)
     prediction_frames, targets = [], []
     cw, ch = (w + 1) // 2, (h + 1) // 2
@@ -52,6 +52,24 @@ def main():
         targets.append((b[:w * h].reshape(h, w).copy(), b[w * h:w * h + cw * ch].reshape(ch, cw).copy(),
                         b[w * h + cw * ch:].reshape(ch, cw).copy()))
         prediction_frames.append(pf)
+    return state, chunk, prediction_frames, targets
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--frames", type=int, default=12)
+    ap.add_argument("--device", type=int, default=0)
+    ap.add_argument("--prev", default=PREV)
+    ap.add_argument("--chunk", default=CHUNK)
+    ap.add_argument("--kf-q-weight", type=float, default=0.75)
+    a = ap.parse_args()
+
+    from alfalfa_b200 import Context, Decoder, Encoder
+    from alfalfa_b200.decoder import read_ivf, write_ivf
+
+    w, h = read_ivf(open(a.chunk, "rb").read())[:2]
+    ctx = Context(w, h, device=a.device, max_frames=32)
+    state, chunk, prediction_frames, targets = bench_inputs(ctx, a.prev, a.chunk, a.frames)
 
     def run():
         enc = Encoder.from_decoder(ctx, Decoder.deserialize(ctx, state))
