@@ -5,4 +5,4 @@ alfalfa_b200/libvp8gpu.so = hand-written sm_90a CUDA kernels + a C++ host librar
 """
 from .capi import CudaError, Invalid, LogicError, Unsupported, Vp8Error  # noqa: F401
 from .decoder import (Context, Decoder, DecoderState, Encoder, FilePlayer, ParsedFrame, RasterHandle,  # noqa: F401
-                      decode_ivf, write_ivf)
+                      decode_ivf, reencode_chunks, write_ivf)

@@ -68,6 +68,12 @@ class EncodeFeatures(C.Structure):
                 ("saved_coef_probs", C.c_void_p)]
 
 
+class ReencodeJob(C.Structure):
+    _fields_ = [("encoder", C.c_void_p), ("y", C.c_void_p), ("u", C.c_void_p), ("v", C.c_void_p), ("y_stride", C.c_size_t),
+                ("uv_stride", C.c_size_t), ("prediction_frame", C.c_void_p), ("y_ac_qi", C.c_int), ("last_frame", C.c_int),
+                ("out", C.c_void_p), ("cap", C.c_size_t), ("size", C.c_size_t), ("status", C.c_int)]
+
+
 class Job(C.Structure):
     _fields_ = [("desc", C.POINTER(FrameDesc)), ("mbs", C.c_void_p), ("tokens", C.c_void_p), ("split", C.c_void_p),
                 ("refs", C.c_int32 * 3), ("out", C.c_int32)]
@@ -149,6 +155,7 @@ SYMBOLS = {
     "vp8gpu_encoder_set_two_pass": (C.c_int, [_vp, C.c_int]),
     "vp8gpu_encoder_update_residues": (C.c_int, [_vp, _u8p, C.c_size_t, _u8p, _u8p, C.c_size_t, _vp, C.c_int, C.c_int,
                                                  _u8p, C.c_size_t, C.POINTER(C.c_size_t)]),
+    "vp8gpu_encoder_update_residues_batch": (C.c_int, [C.POINTER(ReencodeJob), C.c_int]),
     "vp8gpu_encoder_reencode_as_interframe": (C.c_int, [_vp, _u8p, C.c_size_t, _u8p, _u8p, C.c_size_t, _vp, C.c_int,
                                                         _u8p, C.c_size_t, C.POINTER(C.c_size_t)]),
     "vp8gpu_encoder_write_frame": (C.c_int, [_vp, _vp, _u8p, C.c_size_t, C.POINTER(C.c_size_t)]),

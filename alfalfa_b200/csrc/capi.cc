@@ -24,6 +24,7 @@
 
 #include "../../include/vp8gpu.h"
 #include "engine.hpp"
+#include "hostpool.h"
 #include "parser.h"
 #include "serializer.h"
 
@@ -539,6 +540,24 @@ vp8gpu_parsed* next_ring_slot(vp8gpu_decoder* d) {
   return p;
 }
 
+// Frame::copy_to (frame.cc:272-307): the decoder's references after frame `out` (decoded from desc)
+void copy_to_references(vp8gpu_decoder* d, const vp8gpu_frame_desc& desc, int out) {
+  Engine* e = d->ctx->engine;
+  if (desc.key_frame) {
+    set_ref(e, &d->refs[0], out);
+    set_ref(e, &d->refs[1], out);
+    set_ref(e, &d->refs[2], out);
+  } else {
+    if (desc.copy_to_alternate == 1) set_ref(e, &d->refs[2], d->refs[0]);
+    else if (desc.copy_to_alternate == 2) set_ref(e, &d->refs[2], d->refs[1]);
+    if (desc.copy_to_golden == 1) set_ref(e, &d->refs[1], d->refs[0]);
+    else if (desc.copy_to_golden == 2) set_ref(e, &d->refs[1], d->refs[2]);
+    if (desc.refresh_golden) set_ref(e, &d->refs[1], out);
+    if (desc.refresh_alternate) set_ref(e, &d->refs[2], out);
+    if (desc.refresh_last) set_ref(e, &d->refs[0], out);
+  }
+}
+
 // Decoder::decode_frame (decoder.cc:101-118): decode + loopfilter into a fresh raster, then
 // Frame::copy_to (frame.cc:272-307) on the references.
 int decode_parsed_impl(vp8gpu_decoder* d, vp8gpu_parsed* p, bool pinned_ring, int* shown, int* out_id,
@@ -569,19 +588,7 @@ int decode_parsed_impl(vp8gpu_decoder* d, vp8gpu_parsed* p, bool pinned_ring, in
   }
   if (pinned_ring) p->busy = true;
   else cudaStreamSynchronize(e->stream(d->lane));  // caller-owned (possibly pageable) records
-  if (desc.key_frame) {
-    set_ref(e, &d->refs[0], out);
-    set_ref(e, &d->refs[1], out);
-    set_ref(e, &d->refs[2], out);
-  } else {
-    if (desc.copy_to_alternate == 1) set_ref(e, &d->refs[2], d->refs[0]);
-    else if (desc.copy_to_alternate == 2) set_ref(e, &d->refs[2], d->refs[1]);
-    if (desc.copy_to_golden == 1) set_ref(e, &d->refs[1], d->refs[0]);
-    else if (desc.copy_to_golden == 2) set_ref(e, &d->refs[1], d->refs[2]);
-    if (desc.refresh_golden) set_ref(e, &d->refs[1], out);
-    if (desc.refresh_alternate) set_ref(e, &d->refs[2], out);
-    if (desc.refresh_last) set_ref(e, &d->refs[0], out);
-  }
+  copy_to_references(d, desc, out);
   if (shown) *shown = desc.show_frame;
   if (out_id) *out_id = out;  // the allocation's reference goes to the caller
   else e->frame_release(out);
@@ -783,18 +790,24 @@ int vp8gpu_decoder_decode(vp8gpu_decoder* d, const uint8_t* data, size_t len, in
   return rc;
 }
 
-// Internal (encoder.cu, Encoder::write_frame's "decode what was written", encoder.cc:153-158): vp8gpu_decoder_decode
-// of a frame this library has just serialised from `enc_mbs` / `enc_tokens`.  The first partition is parsed like any
-// other frame's (state, modes, vectors, resolved loop-filter levels), but the DCT partitions are not decoded again:
-// their content is the token lists they were written from (tok_off / tok_cnt of the writer's records index
-// enc_tokens; the order inside a macroblock's list does not matter to the kernels).  Saves the serial half of the
-// parse, which is most of a frame's host time.
-int vp8gpu_decoder_decode_known_tokens(vp8gpu_decoder* d, const uint8_t* data, size_t len, const vp8gpu_mb* enc_mbs,
-                                       const vp8gpu_token* enc_tokens, uint32_t n_tok, int* shown, vp8gpu_frame_id* out) {
-  if (!d || !data || !enc_mbs || (n_tok && !enc_tokens)) return VP8GPU_ERR_LOGIC;
+}  // extern "C"
+
+namespace {
+
+// vp8gpu_decoders_decode_written with records: the first partition is parsed like any other frame's (state, modes,
+// vectors, resolved loop-filter levels), but the DCT partitions are not decoded again: their content is the token lists
+// they were written from (tok_off / tok_cnt of the writer's records index enc_tokens; the order inside a macroblock's
+// list does not matter to the kernels).  Saves the serial half of the parse, which is most of a frame's host time.
+int parse_written(vp8gpu_decoder* d, vp8gpu_parsed* p, const uint8_t* data, size_t len, const vp8gpu_mb* enc_mbs,
+                  const vp8gpu_token* enc_tokens, uint32_t n_tok) {
   Engine* e = d->ctx->engine;
-  cudaSetDevice(e->device());
-  vp8gpu_parsed* p = next_ring_slot(d);
+  if (!enc_mbs) {  // the full parse
+    const int rc = vp8::parse_frame(d->state.s, data, len, p->f);
+    if (rc != VP8GPU_OK) return e->fail(rc, "parse_frame failed");
+    count_mbs(p);
+    return VP8GPU_OK;
+  }
+  if (n_tok && !enc_tokens) return VP8GPU_ERR_LOGIC;
   const int rc = vp8::parse_frame(d->state.s, data, len, p->f, true);
   if (rc != VP8GPU_OK) return e->fail(rc, "parse_frame failed");
   const size_t n = (size_t)p->f.desc.mb_cols * p->f.desc.mb_rows;
@@ -814,7 +827,68 @@ int vp8gpu_decoder_decode_known_tokens(vp8gpu_decoder* d, const uint8_t* data, s
   p->f.desc.n_tokens = n_tok;
   p->f.tw.deferred = false;
   count_mbs(p);
-  return decode_parsed_impl(d, p, true, shown, out);
+  return VP8GPU_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+// Internal (encoder.cu, Encoder::write_frame's "decode what was written", encoder.cc:153-158): frame i, just written by
+// this library, decoded by decoder ds[i] -- vp8gpu_decoder_decode of every frame, but the n frames share one set of
+// launches (one Engine::submit on `lane`; < 0: the first decoder's lane) and their first partitions are parsed on the
+// host pool.  enc_mbs[i] / enc_tokens[i] / n_tok[i]: the records and token lists frame i was written from (see
+// parse_written); enc_mbs[i] == nullptr: the full parse.  The decoders must be distinct.  rcs[i]: frame i's status (a
+// refused frame leaves its decoder as it was); returns the first failure or VP8GPU_OK.
+int vp8gpu_decoders_decode_written(vp8gpu_decoder* const* ds, int n, int lane, const uint8_t* const* data, const size_t* len,
+                                   const vp8gpu_mb* const* enc_mbs, const vp8gpu_token* const* enc_tokens, const uint32_t* n_tok,
+                                   int* rcs) {
+  if (n <= 0) return n < 0 ? VP8GPU_ERR_LOGIC : VP8GPU_OK;
+  Engine* e = ds[0]->ctx->engine;
+  cudaSetDevice(e->device());
+  std::vector<vp8gpu_parsed*> ps(n);
+  for (int i = 0; i < n; i++) ps[i] = next_ring_slot(ds[i]);
+  auto parse = [&](int i) { rcs[i] = parse_written(ds[i], ps[i], data[i], len[i], enc_mbs[i], enc_tokens[i], n_tok[i]); };
+  {
+    vp8::HostPool::Group grp;
+    for (int i = 1; i < n; i++) grp.run([&parse, i] { parse(i); });
+    parse(0);
+    grp.wait();
+  }
+  std::vector<HostJob> jobs;
+  std::vector<int> which;
+  for (int i = 0; i < n; i++) {
+    if (rcs[i] != VP8GPU_OK) continue;
+    int out = -1;
+    rcs[i] = e->frame_alloc(&out);
+    if (rcs[i] != VP8GPU_OK) continue;
+    HostJob j;
+    j.desc = &ps[i]->f.desc;
+    j.mbs = ps[i]->f.mbs.data();
+    j.tokens = ps[i]->f.tokens.data();
+    j.split = ps[i]->f.split.data();
+    memcpy(j.refs, ds[i]->refs, sizeof(j.refs));
+    j.out = out;
+    j.n_intra = (int)ps[i]->n_intra;
+    j.n_filtered = (int)ps[i]->n_filtered;
+    j.consumed = ps[i]->consumed;
+    jobs.push_back(j);
+    which.push_back(i);
+  }
+  const int rc = e->submit(lane < 0 ? ds[0]->lane : lane, jobs.data(), (int)jobs.size(), nullptr);
+  for (size_t k = 0; k < jobs.size(); k++) {
+    const int i = which[k];
+    if (rc == VP8GPU_OK) {
+      ps[i]->busy = true;
+      copy_to_references(ds[i], *jobs[k].desc, jobs[k].out);
+    } else {
+      rcs[i] = rc;
+    }
+    e->frame_release(jobs[k].out);
+  }
+  for (int i = 0; i < n; i++)
+    if (rcs[i] != VP8GPU_OK) return rcs[i];
+  return VP8GPU_OK;
 }
 
 int vp8gpu_decoder_decode_parsed(vp8gpu_decoder* d, const vp8gpu_parsed* parsed, int* shown, vp8gpu_frame_id* out) {

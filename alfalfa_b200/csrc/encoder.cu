@@ -21,9 +21,11 @@
 #include <stdlib.h>
 #include <string.h>
 
+#include <algorithm>
 #include <chrono>
 #include <condition_variable>
 #include <mutex>
+#include <string>
 #include <utility>
 #include <vector>
 
@@ -42,8 +44,9 @@ using vp8::Engine;
 extern "C" Engine* vp8gpu_ctx_engine(vp8gpu_ctx* ctx);
 extern "C" int vp8gpu_ctx_next_lane(vp8gpu_ctx* ctx);
 extern "C" const vp8::ParsedFrame* vp8gpu_parsed_frame(const vp8gpu_parsed* p);
-extern "C" int vp8gpu_decoder_decode_known_tokens(vp8gpu_decoder* d, const uint8_t* data, size_t len, const vp8gpu_mb* enc_mbs,
-                                                  const vp8gpu_token* enc_tokens, uint32_t n_tok, int* shown, vp8gpu_frame_id* out);
+extern "C" int vp8gpu_decoders_decode_written(vp8gpu_decoder* const* ds, int n, int lane, const uint8_t* const* data, const size_t* len,
+                                              const vp8gpu_mb* const* enc_mbs, const vp8gpu_token* const* enc_tokens,
+                                              const uint32_t* n_tok, int* rcs);
 
 struct vp8gpu_encoder {
   vp8gpu_ctx* ctx = nullptr;
@@ -580,6 +583,23 @@ static std::mutex g_enc_pool_mu;
 static std::vector<std::pair<Engine*, EncBufferSet>> g_enc_pool;
 constexpr size_t kEncPoolPerEngine = 4;
 
+// job descriptors of one set of re-encode launches: ReencJob[cap] | DevJob[cap] | ticket, pinned and on the device.
+// Kept per context and grown on demand (vp8gpu_encoder_pool_purge frees them with the context).
+struct ReencScratch {
+  int cap = 0;
+  size_t off_dj = 0, off_sync = 0, bytes = 0;
+  uint8_t* host = nullptr;
+  uint8_t* dev = nullptr;
+};
+static std::vector<std::pair<Engine*, ReencScratch*>> g_reenc_scratch;  // idle ones, guarded by g_enc_pool_mu
+
+static void reenc_scratch_free(ReencScratch* sc) {
+  if (sc->host) cudaFreeHost(sc->host);
+  if (sc->dev) cudaFree(sc->dev);
+  delete sc;
+}
+
+
 static void enc_buffers_free(const EncBufferSet& b) {
   if (b.dev) cudaFree(b.dev);
   if (b.d_split) cudaFree(b.d_split);
@@ -595,8 +615,17 @@ static void enc_buffers_free(const EncBufferSet& b) {
 // capi.cc vp8gpu_ctx_destroy: the context's buffer sets die with it
 extern "C" void vp8gpu_encoder_pool_purge(Engine* e) {
   std::vector<EncBufferSet> dead;
+  std::vector<ReencScratch*> dead_scratch;
   {
     std::lock_guard<std::mutex> lk(g_enc_pool_mu);
+    for (size_t i = 0; i < g_reenc_scratch.size();) {
+      if (g_reenc_scratch[i].first == e) {
+        dead_scratch.push_back(g_reenc_scratch[i].second);
+        g_reenc_scratch.erase(g_reenc_scratch.begin() + i);
+      } else {
+        i++;
+      }
+    }
     for (size_t i = 0; i < g_enc_pool.size();) {
       if (g_enc_pool[i].first == e) {
         dead.push_back(g_enc_pool[i].second);
@@ -607,6 +636,7 @@ extern "C" void vp8gpu_encoder_pool_purge(Engine* e) {
     }
   }
   for (const EncBufferSet& b : dead) enc_buffers_free(b);
+  for (ReencScratch* sc : dead_scratch) reenc_scratch_free(sc);
 }
 
 // common part of create / clone / create_from: buffers on device and host, the rate tables
@@ -1245,42 +1275,73 @@ int vp8gpu_encoder_minihash(vp8gpu_encoder* enc, uint32_t* out) {
 
 // Encoder::write_frame's state update (encoder.cc:146-170): decode the emitted frame like any receiver
 // (Frame::decode + loopfilter + copy_to on the device, through the library's own Decoder) and adopt the
-// DecoderState and References it ends with.
-// mbs / tokens: the records and token lists the frame was serialised from (enc->h_mbs / h_tokens), when it was --
-// the decode then skips parsing the DCT partitions back (capi.cc vp8gpu_decoder_decode_known_tokens)
+// DecoderState and References it ends with.  n Encoders at once (update_residues_batch): their frames share one set of
+// decode launches on `lane` (< 0: the lane of the first Encoder's decoder).
+// mbs / tokens: the records and token lists a frame was serialised from (enc->h_mbs / h_tokens), when it was --
+// the decode then skips parsing the DCT partitions back (capi.cc parse_written)
+struct Emitted {
+  const uint8_t* data;
+  size_t len;
+  const vp8gpu_mb* mbs;
+  const vp8gpu_token* tokens;
+  uint32_t n_tok;
+};
+static void apply_emitted_frames(vp8gpu_encoder* const* encs, int n, int lane, const Emitted* fr, int* rcs) {
+  std::vector<vp8gpu_decoder*> ds;
+  std::vector<const uint8_t*> data;
+  std::vector<size_t> len;
+  std::vector<const vp8gpu_mb*> mbs;
+  std::vector<const vp8gpu_token*> toks;
+  std::vector<uint32_t> n_tok;
+  std::vector<int> which, drc;
+  for (int i = 0; i < n; i++) {
+    vp8gpu_decoder* d = nullptr;
+    rcs[i] = vp8gpu_encoder_export_decoder(encs[i], &d);
+    if (rcs[i] != VP8GPU_OK) continue;
+    const bool known = fr[i].mbs && enc_speculate();
+    ds.push_back(d);
+    data.push_back(fr[i].data);
+    len.push_back(fr[i].len);
+    mbs.push_back(known ? fr[i].mbs : nullptr);
+    toks.push_back(known ? fr[i].tokens : nullptr);
+    n_tok.push_back(known ? fr[i].n_tok : 0);
+    which.push_back(i);
+  }
+  drc.assign(ds.size(), VP8GPU_OK);
+  vp8gpu_decoders_decode_written(ds.data(), (int)ds.size(), lane, data.data(), len.data(), mbs.data(), toks.data(), n_tok.data(),
+                                 drc.data());
+  for (size_t k = 0; k < ds.size(); k++) {
+    vp8gpu_encoder* enc = encs[which[k]];
+    vp8gpu_decoder* d = ds[k];
+    int rc = drc[k];
+    if (rc == VP8GPU_OK) {
+      const vp8gpu_state* st = vp8gpu_decoder_state(d);
+      std::vector<uint8_t> blob(vp8gpu_state_serialize(st, nullptr, 0));
+      vp8gpu_state_serialize(st, blob.data(), blob.size());
+      if (!vp8::State::deserialize(blob.data(), blob.size(), *enc->dec_state)) rc = enc->e->fail(VP8GPU_ERR_LOGIC, "write_frame: bad decoder state");
+    }
+    if (rc == VP8GPU_OK) {
+      vp8gpu_frame_id refs[3];
+      vp8gpu_decoder_references(d, refs);
+      for (int r = 0; r < 3; r++)
+        if (refs[r] >= 0) enc->e->frame_retain(refs[r]);
+      for (int r = 0; r < 3; r++) {
+        if (enc->refs[r] >= 0) enc->e->frame_release(enc->refs[r]);
+        enc->refs[r] = refs[r];
+      }
+      enc->has_state = true;
+      enc->stat_frames++;
+    }
+    rcs[which[k]] = rc;
+    vp8gpu_decoder_destroy(d);
+  }
+}
+
 static int apply_emitted_frame(vp8gpu_encoder* enc, const uint8_t* data, size_t len, const vp8gpu_mb* mbs, const vp8gpu_token* tokens,
                                uint32_t n_tok) {
-  Engine* e = enc->e;
-  vp8gpu_decoder* d = nullptr;
-  int rc = vp8gpu_encoder_export_decoder(enc, &d);
-  if (rc != VP8GPU_OK) return rc;
-  int shown = 0;
-  vp8gpu_frame_id raster = -1;
-  if (mbs && enc_speculate()) rc = vp8gpu_decoder_decode_known_tokens(d, data, len, mbs, tokens, n_tok, &shown, &raster);
-  else rc = vp8gpu_decoder_decode(d, data, len, &shown, &raster);
-  if (rc == VP8GPU_OK) {
-    if (raster >= 0) e->frame_release(raster);
-    const std::vector<uint8_t> blob = [&] {
-      const vp8gpu_state* st = vp8gpu_decoder_state(d);
-      std::vector<uint8_t> b(vp8gpu_state_serialize(st, nullptr, 0));
-      vp8gpu_state_serialize(st, b.data(), b.size());
-      return b;
-    }();
-    if (!vp8::State::deserialize(blob.data(), blob.size(), *enc->dec_state)) rc = e->fail(VP8GPU_ERR_LOGIC, "write_frame: bad decoder state");
-  }
-  if (rc == VP8GPU_OK) {
-    vp8gpu_frame_id refs[3];
-    vp8gpu_decoder_references(d, refs);
-    for (int k = 0; k < 3; k++)
-      if (refs[k] >= 0) e->frame_retain(refs[k]);
-    for (int k = 0; k < 3; k++) {
-      if (enc->refs[k] >= 0) e->frame_release(enc->refs[k]);
-      enc->refs[k] = refs[k];
-    }
-    enc->has_state = true;
-    enc->stat_frames++;
-  }
-  vp8gpu_decoder_destroy(d);
+  const Emitted fr = {data, len, mbs, tokens, n_tok};
+  int rc = VP8GPU_OK;
+  apply_emitted_frames(&enc, 1, -1, &fr, &rc);
   return rc;
 }
 
@@ -1310,14 +1371,42 @@ int vp8gpu_encoder_write_frame(vp8gpu_encoder* enc, const vp8gpu_parsed* frame, 
   return rc;
 }
 
-// Encoder::update_residues + write_frame (encoder/reencode.cc:131-313): the prediction frame's modes, vectors,
-// references and header are kept, its residues are recomputed against THIS encoder's references so that the frame
-// decodes close to the target raster; y_ac_qi < 0 keeps the frame's own quantiser index (the deltas always stay).
-int vp8gpu_encoder_update_residues(vp8gpu_encoder* enc, const uint8_t* y, size_t y_stride, const uint8_t* u, const uint8_t* v,
-                                   size_t uv_stride, const vp8gpu_parsed* prediction_frame, int y_ac_qi, int last_frame, uint8_t* out,
-                                   size_t cap, size_t* size) {
-  const vp8::ParsedFrame* pf = vp8gpu_parsed_frame(prediction_frame);
-  if (!enc || !y || !u || !v || !pf || !size || y_ac_qi > 127) return VP8GPU_ERR_LOGIC;
+}  // extern "C"
+
+// ---- Encoder::update_residues + write_frame (encoder/reencode.cc:131-313) -------------------------------------------
+// The prediction frame's modes, vectors, references and header are kept, its residues are recomputed against THIS
+// encoder's references so that the frame decodes close to the target raster; y_ac_qi < 0 keeps the frame's own quantiser
+// index (the deltas always stay).  One call or a batch of independent Encoders of one context go through the same steps:
+// prepare (validation, the target upload, the quantiser, the records), one set of launches for all of them on one lane,
+// then the writer and the decode of the emitted frames that advances every Encoder.
+namespace {
+
+struct ReencTask {
+  vp8gpu_encoder* enc = nullptr;
+  const vp8::ParsedFrame* pf = nullptr;
+  const uint8_t *y = nullptr, *u = nullptr, *v = nullptr;
+  size_t y_stride = 0, uv_stride = 0;
+  int y_ac_qi = -1, last_frame = 0;
+  uint8_t* out = nullptr;
+  size_t cap = 0;
+  size_t* size = nullptr;
+  // filled in by the steps
+  int qi = 0;
+  vp8gpu_quant q{};
+  size_t n_intra = 0, split_bytes = 0;
+  int recon = -1;
+  uint32_t n_tok = 0;
+  std::vector<uint8_t> bytes;
+  bool launched = false;  // got past its validation: its Encoder took part in the launches
+  int rc = VP8GPU_OK;
+  std::string err;        // the message of its failure (the context's last error may be another job's)
+};
+
+// step 1 (host): everything of one job that the launches need, and every refusal of the single call
+int reenc_prepare(ReencTask& t) {
+  vp8gpu_encoder* enc = t.enc;
+  const vp8::ParsedFrame* pf = t.pf;
+  if (!enc || !t.y || !t.u || !t.v || !pf || !t.size || t.y_ac_qi > 127) return VP8GPU_ERR_LOGIC;
   Engine* e = enc->e;
   const vp8::Geom& g = e->geom();
   const vp8::Verbatim& vb = pf->verbatim;
@@ -1334,13 +1423,11 @@ int vp8gpu_encoder_update_residues(vp8gpu_encoder* enc, const uint8_t* y, size_t
   // update is reproduced as it is: one Quantizer for the residues (reencode.cc:283) whatever the segments say.
   if (vb.read_segment) return e->fail(VP8GPU_ERR_UNSUPPORTED, "update_residues: the prediction frame updates the segment map");
   cudaSetDevice(e->device());
-  int rc = upload_source(enc, y, y_stride, u, v, uv_stride);
+  int rc = upload_source(enc, t.y, t.y_stride, t.u, t.v, t.uv_stride);
   if (rc != VP8GPU_OK) return rc;
-  if (int lrc = e->ensure_lane(enc->lane)) return lrc;
-  cudaStream_t s = e->stream(enc->lane);
 
-  const int qi = y_ac_qi < 0 ? vb.y_ac_qi : y_ac_qi;
-  vp8gpu_quant q;  // Quantizer::Quantizer (quantization.cc:83-93) of the frame's indices with y_ac_qi replaced
+  const int qi = t.y_ac_qi < 0 ? vb.y_ac_qi : t.y_ac_qi;
+  vp8gpu_quant& q = t.q;  // Quantizer::Quantizer (quantization.cc:83-93) of the frame's indices with y_ac_qi replaced
   q.y_ac = k_ac_q[clamp_q(qi)];
   q.y_dc = k_dc_q[clamp_q(qi + vb.q_delta[0])];
   q.y2_dc = static_cast<uint16_t>(k_dc_q[clamp_q(qi + vb.q_delta[1])] * 2);
@@ -1349,122 +1436,225 @@ int vp8gpu_encoder_update_residues(vp8gpu_encoder* enc, const uint8_t* y, size_t
   q.uv_ac = k_ac_q[clamp_q(qi + vb.q_delta[4])];
   if (q.y2_ac < 8) q.y2_ac = 8;
   if (q.uv_dc > 132) q.uv_dc = 132;
+  t.qi = qi;
 
   // records: the frame's, with empty token lists (step 1 predicts, steps 2 and 4 fill the lists in)
-  size_t n_intra = 0;
+  t.n_intra = 0;
   for (size_t i = 0; i < n_mbs; i++) {
     vp8gpu_mb m = pf->mbs.data()[i];
     m.tok_off = 0;
     m.tok_cnt = 0;
     m.flags = (m.y_mode != VP8GPU_B_PRED && m.y_mode != VP8GPU_SPLITMV) ? VP8GPU_MB_HAS_Y2 : 0;
     if (m.y_mode == VP8GPU_SPLITMV && m.split_idx >= pf->desc.n_split) return e->fail(VP8GPU_ERR_LOGIC, "update_residues: bad split index");
-    n_intra += m.ref_frame == VP8GPU_REF_CURRENT;
+    t.n_intra += m.ref_frame == VP8GPU_REF_CURRENT;
     enc->h_mbs[i] = m;
   }
-  const size_t split_bytes = (size_t)pf->desc.n_split * sizeof(vp8gpu_split_mvs);
-  if (split_bytes > enc->split_cap) {
+  t.split_bytes = (size_t)pf->desc.n_split * sizeof(vp8gpu_split_mvs);
+  if (t.split_bytes > enc->split_cap) {
     if (enc->d_split) cudaFree(enc->d_split);
     enc->d_split = nullptr;
     enc->split_cap = 0;
     if (cudaMalloc(&enc->d_split, n_mbs * sizeof(vp8gpu_split_mvs)) != cudaSuccess) return e->fail(VP8GPU_ERR_NOMEM, "update_residues: split buffer");
     enc->split_cap = n_mbs * sizeof(vp8gpu_split_mvs);
   }
+  return e->frame_alloc(&t.recon);
+}
 
-  int recon = -1;
-  rc = e->frame_alloc(&recon);
-  if (rc != VP8GPU_OK) return rc;
-  auto fail = [&](int code) {
-    e->frame_release(recon);
+// step 2 (device): one k_inter (prediction), k_reenc_inter, k_inter (reconstruction) and k_reenc_intra for all jobs on
+// `lane`, then their records and token lists back on the host.  Every job has its own target, reconstruction, records,
+// token pool and counters (its Encoder's buffers); launches that no job needs are skipped.  A job whose token pool
+// overflowed gets its own status; any other failure is the launch's and fails every job.  Releases the reconstructions.
+int reenc_launch(ReencTask* const* ts, int n, int lane) {
+  Engine* e = ts[0]->enc->e;
+  const vp8::Geom& g = e->geom();
+  const size_t n_mbs = (size_t)g.mb_cols * g.mb_rows;
+  ReencScratch* sc = nullptr;
+  cudaStream_t s = nullptr;
+  Engine::thread_error().clear();
+  auto done = [&](int code) {
+    for (int i = 0; i < n; i++) {
+      e->frame_release(ts[i]->recon);
+      ts[i]->recon = -1;
+      if (code != VP8GPU_OK) {
+        ts[i]->rc = code;
+        ts[i]->err = Engine::thread_error();
+      }
+    }
+    // after a failure, copies out of the scratch's pinned descriptors may still be queued: the next user of the scratch
+    // rewrites them, so the lane drains first (its own status no longer matters)
+    if (sc && code != VP8GPU_OK && s) cudaStreamSynchronize(s);
+    if (sc) {
+      std::lock_guard<std::mutex> lk(g_enc_pool_mu);
+      g_reenc_scratch.emplace_back(e, sc);
+    }
     return code;
   };
-  int ids[5] = {enc->src, recon, enc->refs[0], -1, -1};
-  int n_ids = 3;
-  for (int k = 1; k < 3; k++) {
-    bool dup = false;
-    for (int j = 2; j < n_ids; j++) dup |= ids[j] == enc->refs[k];
-    if (!dup) ids[n_ids++] = enc->refs[k];
-  }
-  rc = e->acquire_frames(enc->lane, ids, n_ids, 2u);  // only `recon` is written
-  if (rc != VP8GPU_OK) return fail(rc);
-
-  memset(enc->h_hdr, 0, 1024);
-  vp8::ReencJob* rj = reinterpret_cast<vp8::ReencJob*>(enc->h_hdr);
-  vp8::DevJob* dj = reinterpret_cast<vp8::DevJob*>(enc->h_hdr + 512);
-  int* d_sync = reinterpret_cast<int*>(enc->dev + enc->off_sync);
-  vp8gpu_mb* d_mbs = reinterpret_cast<vp8gpu_mb*>(enc->dev + enc->off_mbs);
-  vp8gpu_token* d_tok = reinterpret_cast<vp8gpu_token*>(enc->dev + enc->off_tokens);
-  rj->target = e->frame_dev(enc->src);
-  rj->recon = e->frame_dev(recon);
-  rj->mbs_in = d_mbs;
-  rj->mbs_out = d_mbs;
-  rj->tokens = d_tok;
-  rj->tok_counter = reinterpret_cast<uint32_t*>(d_sync + 96);
-  rj->tok_cap = enc->tok_cap;
-  rj->progress = d_sync + 128;
-  rj->q = q;
-  rj->cols = (uint16_t)g.mb_cols;
-  rj->rows = (uint16_t)g.mb_rows;
-  dj->mbs = d_mbs;
-  dj->tokens = d_tok;
-  dj->split = reinterpret_cast<const vp8gpu_split_mvs*>(enc->d_split);
-  dj->out = e->frame_dev(recon);
-  for (int k = 0; k < 3; k++) {
-    dj->ref[k] = e->frame_dev(enc->refs[k]);
-    dj->ref_tmap[k] = e->frame_tmaps(enc->refs[k]);
-  }
-  dj->intra_progress = d_sync + 128;
-  dj->lf_progress = d_sync + 128 + g.mb_rows;
-  for (int k = 0; k < 4; k++) dj->quant[k] = q;
 #define CUF(call)                                                        \
   do {                                                                   \
     cudaError_t e__ = (call);                                            \
-    if (e__ != cudaSuccess) return fail(e->cuda_fail(e__, #call));       \
+    if (e__ != cudaSuccess) return done(e->cuda_fail(e__, #call));       \
   } while (0)
-  CUF(cudaMemcpyAsync(enc->dev + enc->off_encjob, enc->h_hdr, 1024, cudaMemcpyHostToDevice, s));
-  CUF(cudaMemcpyAsync(d_mbs, enc->h_mbs, n_mbs * sizeof(vp8gpu_mb), cudaMemcpyHostToDevice, s));
-  if (split_bytes) CUF(cudaMemcpyAsync(enc->d_split, pf->split.data(), split_bytes, cudaMemcpyHostToDevice, s));
-  CUF(cudaMemsetAsync(d_sync, 0, sizeof(int) * (128 + 2 * (size_t)g.mb_rows), s));
-  const vp8::ReencJob* d_rj = reinterpret_cast<const vp8::ReencJob*>(enc->dev + enc->off_encjob);
-  const vp8::DevJob* d_dj = reinterpret_cast<const vp8::DevJob*>(enc->dev + enc->off_encjob + 512);
+  if (int rc = e->ensure_lane(lane)) return done(rc);
+  s = e->stream(lane);
+  // The Encoders' records, token pools, counters and split-MV buffers are used below on `lane`, so work an Encoder
+  // queued on its own lane comes first.  They are not rasters with events of their own, and every Encoder call ends with
+  // its lane drained (it waits for its results), so a host synchronisation of the other lanes returns at once and costs
+  // nothing; it is only there so that the batch stays correct if that ever changes.
+  for (int i = 0; i < n; i++) {
+    const int l = ts[i]->enc->lane;
+    if (l != lane && e->stream(l)) CUF(cudaStreamSynchronize(e->stream(l)));
+  }
+  // the rasters, each once (clones and Encoders made from one Decoder share references): only the reconstructions
+  // are written; acquired in groups of 32 (the width of the write mask)
+  std::vector<int> ids;
+  std::vector<uint8_t> written;
+  auto add = [&](int id, bool w) {
+    for (int x : ids)
+      if (x == id) return;
+    ids.push_back(id);
+    written.push_back(w);
+  };
+  bool any_inter = false, any_intra = false;
+  for (int i = 0; i < n; i++) {
+    const vp8gpu_encoder* enc = ts[i]->enc;
+    add(enc->src, false);
+    add(ts[i]->recon, true);
+    for (int k = 0; k < 3; k++) add(enc->refs[k], false);
+    any_inter |= ts[i]->n_intra < n_mbs;
+    any_intra |= ts[i]->n_intra != 0;
+  }
+  auto in_groups = [&](bool acquire) {
+    for (size_t k = 0; k < ids.size(); k += 32) {
+      const int m = (int)std::min<size_t>(32, ids.size() - k);
+      uint32_t mask = 0;
+      for (int j = 0; j < m; j++) mask |= (uint32_t)written[k + j] << j;
+      const int rc = acquire ? e->acquire_frames(lane, ids.data() + k, m, mask) : e->mark_frames(lane, ids.data() + k, m, mask);
+      if (rc != VP8GPU_OK) return rc;
+    }
+    return (int)VP8GPU_OK;
+  };
+  if (int rc = in_groups(true)) return done(rc);
+
+  {
+    std::lock_guard<std::mutex> lk(g_enc_pool_mu);
+    for (size_t i = g_reenc_scratch.size(); i-- > 0;)
+      if (g_reenc_scratch[i].first == e) {
+        sc = g_reenc_scratch[i].second;
+        g_reenc_scratch.erase(g_reenc_scratch.begin() + i);
+        break;
+      }
+  }
+  if (!sc) sc = new ReencScratch();
+  if (sc->cap < n) {
+    if (sc->host) cudaFreeHost(sc->host);
+    if (sc->dev) cudaFree(sc->dev);
+    sc->host = sc->dev = nullptr;
+    sc->cap = 0;
+    const int cap = std::max(n, 8);
+    sc->off_dj = align_up(sizeof(vp8::ReencJob) * cap, 256);
+    sc->off_sync = align_up(sc->off_dj + sizeof(vp8::DevJob) * cap, 256);
+    sc->bytes = sc->off_sync + 256;
+    if (cudaHostAlloc(&sc->host, sc->off_sync, cudaHostAllocDefault) != cudaSuccess || cudaMalloc(&sc->dev, sc->bytes) != cudaSuccess)
+      return done(e->fail(VP8GPU_ERR_NOMEM, "update_residues: job descriptors"));
+    sc->cap = cap;
+  }
+  memset(sc->host, 0, sc->off_sync);
+  vp8::ReencJob* rjs = reinterpret_cast<vp8::ReencJob*>(sc->host);
+  vp8::DevJob* djs = reinterpret_cast<vp8::DevJob*>(sc->host + sc->off_dj);
+  for (int i = 0; i < n; i++) {
+    ReencTask& t = *ts[i];
+    vp8gpu_encoder* enc = t.enc;
+    int* d_sync = reinterpret_cast<int*>(enc->dev + enc->off_sync);
+    vp8gpu_mb* d_mbs = reinterpret_cast<vp8gpu_mb*>(enc->dev + enc->off_mbs);
+    vp8gpu_token* d_tok = reinterpret_cast<vp8gpu_token*>(enc->dev + enc->off_tokens);
+    vp8::ReencJob* rj = rjs + i;
+    rj->target = e->frame_dev(enc->src);
+    rj->recon = e->frame_dev(t.recon);
+    rj->mbs_in = d_mbs;
+    rj->mbs_out = d_mbs;
+    rj->tokens = d_tok;
+    rj->tok_counter = reinterpret_cast<uint32_t*>(d_sync + 96);
+    rj->tok_cap = enc->tok_cap;
+    rj->progress = d_sync + 128;
+    rj->q = t.q;
+    rj->cols = (uint16_t)g.mb_cols;
+    rj->rows = (uint16_t)g.mb_rows;
+    vp8::DevJob* dj = djs + i;
+    dj->mbs = d_mbs;
+    dj->tokens = d_tok;
+    dj->split = reinterpret_cast<const vp8gpu_split_mvs*>(enc->d_split);
+    dj->out = e->frame_dev(t.recon);
+    for (int k = 0; k < 3; k++) {
+      dj->ref[k] = e->frame_dev(enc->refs[k]);
+      dj->ref_tmap[k] = e->frame_tmaps(enc->refs[k]);
+    }
+    dj->intra_progress = d_sync + 128;
+    dj->lf_progress = d_sync + 128 + g.mb_rows;
+    for (int k = 0; k < 4; k++) dj->quant[k] = t.q;
+    CUF(cudaMemcpyAsync(d_mbs, enc->h_mbs, n_mbs * sizeof(vp8gpu_mb), cudaMemcpyHostToDevice, s));
+    if (t.split_bytes) CUF(cudaMemcpyAsync(enc->d_split, t.pf->split.data(), t.split_bytes, cudaMemcpyHostToDevice, s));
+    CUF(cudaMemsetAsync(d_sync, 0, sizeof(int) * (128 + 2 * (size_t)g.mb_rows), s));
+  }
+  int* ticket = reinterpret_cast<int*>(sc->dev + sc->off_sync);
+  CUF(cudaMemcpyAsync(sc->dev, sc->host, sc->off_sync, cudaMemcpyHostToDevice, s));
+  CUF(cudaMemsetAsync(ticket, 0, sizeof(int), s));
+  const vp8::ReencJob* d_rj = reinterpret_cast<const vp8::ReencJob*>(sc->dev);
+  const vp8::DevJob* d_dj = reinterpret_cast<const vp8::DevJob*>(sc->dev + sc->off_dj);
   int launches = 0;
-  if (n_intra < n_mbs) {
-    if (int ce = vp8::launch_inter(d_dj, 1, g, s)) return fail(e->cuda_fail((cudaError_t)ce, "k_inter (prediction)"));
-    if (int ce = vp8::launch_reenc_inter(d_rj, (int)n_mbs, g, s)) return fail(e->cuda_fail((cudaError_t)ce, "k_reenc_inter"));
-    if (int ce = vp8::launch_inter(d_dj, 1, g, s)) return fail(e->cuda_fail((cudaError_t)ce, "k_inter (reconstruction)"));
+  if (any_inter) {
+    if (int ce = vp8::launch_inter(d_dj, n, g, s)) return done(e->cuda_fail((cudaError_t)ce, "k_inter (prediction)"));
+    if (int ce = vp8::launch_reenc_inter(d_rj, n, (int)n_mbs, g, s)) return done(e->cuda_fail((cudaError_t)ce, "k_reenc_inter"));
+    if (int ce = vp8::launch_inter(d_dj, n, g, s)) return done(e->cuda_fail((cudaError_t)ce, "k_inter (reconstruction)"));
     launches += 3;
   }
-  if (n_intra) {
-    if (int ce = vp8::launch_reenc_intra(d_rj, g.mb_rows, g, d_sync + 0, s)) return fail(e->cuda_fail((cudaError_t)ce, "k_reenc_intra"));
+  if (any_intra) {
+    if (int ce = vp8::launch_reenc_intra(d_rj, n, g.mb_rows, g, ticket, s)) return done(e->cuda_fail((cudaError_t)ce, "k_reenc_intra"));
     launches++;
   }
   e->count_launches(launches);
-  e->mark_frames(enc->lane, ids, n_ids, 2u);
-  CUF(cudaMemcpyAsync(enc->h_count, rj->tok_counter, sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
-  CUF(cudaMemcpyAsync(enc->h_mbs, d_mbs, n_mbs * sizeof(vp8gpu_mb), cudaMemcpyDeviceToHost, s));
-  CUF(cudaStreamSynchronize(s));
-  const uint32_t n_tok = *enc->h_count;
-  if (n_tok > enc->tok_cap) return fail(e->fail(VP8GPU_ERR_NOMEM, "update_residues: token pool overflow"));
-  if (n_tok) {
-    CUF(cudaMemcpyAsync(enc->h_tokens, d_tok, (size_t)n_tok * sizeof(vp8gpu_token), cudaMemcpyDeviceToHost, s));
-    CUF(cudaStreamSynchronize(s));
+  if (int rc = in_groups(false)) return done(rc);
+  for (int i = 0; i < n; i++) {
+    vp8gpu_encoder* enc = ts[i]->enc;
+    CUF(cudaMemcpyAsync(enc->h_count, rjs[i].tok_counter, sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
+    CUF(cudaMemcpyAsync(enc->h_mbs, rjs[i].mbs_out, n_mbs * sizeof(vp8gpu_mb), cudaMemcpyDeviceToHost, s));
   }
+  CUF(cudaStreamSynchronize(s));
+  bool any_tokens = false;
+  for (int i = 0; i < n; i++) {
+    ReencTask& t = *ts[i];
+    t.n_tok = *t.enc->h_count;
+    if (t.n_tok > t.enc->tok_cap) {
+      t.rc = e->fail(VP8GPU_ERR_NOMEM, "update_residues: token pool overflow");
+      t.err = "update_residues: token pool overflow";
+    } else if (t.n_tok) {
+      CUF(cudaMemcpyAsync(t.enc->h_tokens, rjs[i].tokens, (size_t)t.n_tok * sizeof(vp8gpu_token), cudaMemcpyDeviceToHost, s));
+      any_tokens = true;
+    }
+  }
+  if (any_tokens) CUF(cudaStreamSynchronize(s));
 #undef CUF
-  e->frame_release(recon);  // the reference discards its reconstruction too: write_frame decodes the frame it wrote
+  // the reference discards its reconstruction too: write_frame decodes the frame it wrote
+  return done(VP8GPU_OK);
+}
 
-  // ---- the frame: header sections of the prediction frame + the reference Encoder's probability decisions ----
+// step 3a (host): the frame -- header sections of the prediction frame + the reference Encoder's probability decisions
+int reenc_write(ReencTask& t) {
+  vp8gpu_encoder* enc = t.enc;
+  Engine* e = enc->e;
+  const vp8::Verbatim& vb = t.pf->verbatim;
   vp8::EncodeHeader h;
   h.key_frame = false;
   h.show_frame = true;  // InterFrame( width, height ): a new frame object is shown
   h.width = e->width();
   h.height = e->height();
-  h.y_ac_qi = qi;
+  h.y_ac_qi = t.qi;
   vp8::EncodeFeatures ft;
   vp8::EncodeFeatures::RefWriterState fresh;  // update_residues builds a new InterFrame object every time
   fresh.prob_last = vb.prob_last;              // prob_references_* are copied from the prediction frame (reencode.cc:266-267)
   fresh.prob_golden = vb.prob_golden;
   ft.ref_writer = &fresh;
   ft.residue_of = &vb;
-  ft.residue_refresh_all = last_frame != 0;
+  ft.residue_refresh_all = t.last_frame != 0;
   ft.log2_partitions = 0;
   uint8_t probs[1056];
   memcpy(probs, enc->dec_state->coef_probs, 1056);
@@ -1472,14 +1662,139 @@ int vp8gpu_encoder_update_residues(vp8gpu_encoder* enc, const uint8_t* y, size_t
   ft.ymode_probs = enc->dec_state->ymode_probs;
   ft.uvmode_probs = enc->dec_state->uvmode_probs;
   ft.mv_probs = enc->dec_state->mv_probs;
-  const std::vector<uint8_t> bytes = vp8::serialize_frame(h, enc->h_mbs, enc->h_tokens, pf->split.data(), &ft);
-  if (bytes.empty()) return e->fail(VP8GPU_ERR_LOGIC, "update_residues: serializer rejected the records");
-  rc = emit(enc, bytes, out, cap, size, enc->h_mbs, enc->h_tokens, n_tok);
-  if (rc == VP8GPU_OK) {  // write_frame, REALTIME_QUALITY (encoder.cc:164-167)
-    enc->last_qi = qi;
-    enc->last_lf = vb.lf_level;
+  t.bytes = vp8::serialize_frame(h, enc->h_mbs, enc->h_tokens, t.pf->split.data(), &ft);
+  if (t.bytes.empty()) return e->fail(VP8GPU_ERR_LOGIC, "update_residues: serializer rejected the records");
+  *t.size = t.bytes.size();
+  if (!t.out || t.cap < t.bytes.size()) return e->fail(VP8GPU_ERR_NOMEM, "output buffer too small");
+  memcpy(t.out, t.bytes.data(), t.bytes.size());
+  return VP8GPU_OK;
+}
+
+// fn(i) for i < n, on the host pool when there is more than one
+template <class F>
+void for_each_job(int n, F fn) {
+  vp8::HostPool::Group grp;
+  for (int i = 1; i < n; i++) grp.run([&fn, i] { fn(i); });
+  if (n > 0) fn(0);
+  grp.wait();
+}
+
+// t.rc = what a step of the task returned, t.err = its failure's message, taken on the thread that ran the step
+template <class F>
+void run_step(ReencTask& t, F step) {
+  Engine::thread_error().clear();
+  t.rc = step();
+  if (t.rc != VP8GPU_OK) t.err = Engine::thread_error();
+}
+
+// the three steps for n jobs of distinct Encoders of one context; t.rc = each job's status.  tl (optional, 8 slots):
+// [0] upload, [3] kernels + download, [5] writer, [6] state update, [7] total.
+void reenc_run(ReencTask* ts, int n, double* tl) {
+  const double t0 = now_ms();
+  for_each_job(n, [ts](int i) { run_step(ts[i], [&] { return reenc_prepare(ts[i]); }); });
+  std::vector<ReencTask*> run;
+  for (int i = 0; i < n; i++)
+    if (ts[i].rc == VP8GPU_OK) {
+      ts[i].launched = true;
+      run.push_back(&ts[i]);
+    }
+  const double t1 = now_ms();
+  if (!run.empty()) reenc_launch(run.data(), (int)run.size(), run[0]->enc->lane);
+  const double t2 = now_ms();
+  for_each_job((int)run.size(), [&run](int i) {
+    if (run[i]->rc == VP8GPU_OK) run_step(*run[i], [&] { return reenc_write(*run[i]); });
+  });
+  const double t3 = now_ms();
+  std::vector<vp8gpu_encoder*> encs;
+  std::vector<Emitted> frames;
+  std::vector<ReencTask*> written;
+  for (ReencTask* t : run)
+    if (t->rc == VP8GPU_OK) {
+      encs.push_back(t->enc);
+      frames.push_back(Emitted{t->bytes.data(), t->bytes.size(), t->enc->h_mbs, t->enc->h_tokens, t->n_tok});
+      written.push_back(t);
+    }
+  std::vector<int> rcs(encs.size(), VP8GPU_OK);
+  Engine::thread_error().clear();
+  if (!encs.empty()) apply_emitted_frames(encs.data(), (int)encs.size(), run[0]->enc->lane, frames.data(), rcs.data());
+  for (size_t k = 0; k < written.size(); k++) {
+    written[k]->rc = rcs[k];
+    if (rcs[k] == VP8GPU_OK) {  // write_frame, REALTIME_QUALITY (encoder.cc:164-167)
+      written[k]->enc->last_qi = written[k]->qi;
+      written[k]->enc->last_lf = written[k]->pf->verbatim.lf_level;
+    } else {
+      written[k]->err = Engine::thread_error();
+    }
   }
-  return rc;
+  const double t4 = now_ms();
+  if (tl) {
+    for (int k = 0; k < 8; k++) tl[k] = 0;
+    tl[0] = t1 - t0;
+    tl[3] = t2 - t1;
+    tl[5] = t3 - t2;
+    tl[6] = t4 - t3;
+    tl[7] = t4 - t0;
+  }
+}
+
+}  // namespace
+
+extern "C" {
+
+int vp8gpu_encoder_update_residues(vp8gpu_encoder* enc, const uint8_t* y, size_t y_stride, const uint8_t* u, const uint8_t* v,
+                                   size_t uv_stride, const vp8gpu_parsed* prediction_frame, int y_ac_qi, int last_frame, uint8_t* out,
+                                   size_t cap, size_t* size) {
+  ReencTask t;
+  t.enc = enc;
+  t.pf = vp8gpu_parsed_frame(prediction_frame);
+  t.y = y, t.u = u, t.v = v, t.y_stride = y_stride, t.uv_stride = uv_stride;
+  t.y_ac_qi = y_ac_qi, t.last_frame = last_frame;
+  t.out = out, t.cap = cap, t.size = size;
+  reenc_run(&t, 1, nullptr);  // (the timeline keeps describing the last encode call, as it always has)
+  return t.rc;
+}
+
+// update_residues of n independent Encoders of one context in one set of launches (include/vp8gpu.h)
+int vp8gpu_encoder_update_residues_batch(vp8gpu_reencode_job* jobs, int n) {
+  if (n < 0 || (n > 0 && !jobs)) return VP8GPU_ERR_LOGIC;
+  // whole-call refusals: an Encoder's frames depend on each other, and one set of launches serves one context
+  Engine* e = nullptr;
+  const char* why = nullptr;
+  for (int i = 0; i < n; i++) {
+    const vp8gpu_encoder* enc = jobs[i].encoder;
+    if (!enc) continue;
+    if (!e) e = enc->e;
+    else if (enc->e != e) why = "update_residues_batch: the encoders belong to different contexts";
+    for (int j = 0; j < i; j++)
+      if (jobs[j].encoder == enc) why = "update_residues_batch: the same encoder appears twice";
+  }
+  if (why) {
+    for (int i = 0; i < n; i++) jobs[i].status = VP8GPU_ERR_LOGIC;
+    return e->fail(VP8GPU_ERR_LOGIC, why);
+  }
+  std::vector<ReencTask> ts(n);
+  for (int i = 0; i < n; i++) {
+    const vp8gpu_reencode_job& j = jobs[i];
+    ReencTask& t = ts[i];
+    t.enc = j.encoder;
+    t.pf = vp8gpu_parsed_frame(j.prediction_frame);
+    t.y = j.y, t.u = j.u, t.v = j.v, t.y_stride = j.y_stride, t.uv_stride = j.uv_stride;
+    t.y_ac_qi = j.y_ac_qi, t.last_frame = j.last_frame;
+    t.out = j.out, t.cap = j.cap, t.size = &jobs[i].size;
+  }
+  double tl[8];
+  reenc_run(ts.data(), n, tl);
+  int first = -1;
+  for (int i = 0; i < n; i++) {
+    jobs[i].status = ts[i].rc;
+    if (ts[i].launched) memcpy(ts[i].enc->tl, tl, sizeof(tl));
+    if (first < 0 && ts[i].rc != VP8GPU_OK) first = i;
+  }
+  if (first < 0) return VP8GPU_OK;
+  // the context's last error names the job whose status is returned (the jobs' steps ran on several host threads)
+  const std::string what = "update_residues_batch: job " + std::to_string(first) + " of " + std::to_string(n) + " failed" +
+                           (ts[first].err.empty() ? std::string() : ": " + ts[first].err);
+  return e ? e->fail(ts[first].rc, what) : ts[first].rc;
 }
 
 // Encoder::reencode_as_interframe + write_frame (encoder/reencode.cc:39-129, 343-351): the chunk's initial key

@@ -48,14 +48,20 @@ constexpr int kSyncHeaderInts = 64;  // [0] = intra ticket, [32] = loop-filter t
 }  // namespace
 
 // workers and dispatchers of vp8gpu_decode_ivf report errors concurrently: the text has its own lock
+std::string& Engine::thread_error() {
+  thread_local std::string err;
+  return err;
+}
 int Engine::fail(int code, const std::string& what) {
   std::lock_guard<std::mutex> lk(err_mu_);
   err_ = what;
+  thread_error() = what;
   return code;
 }
 int Engine::cuda_fail(cudaError_t e, const char* what) {
   std::lock_guard<std::mutex> lk(err_mu_);
   err_ = std::string(what) + ": " + cudaGetErrorString(e);
+  thread_error() = err_;
   return VP8GPU_ERR_CUDA;
 }
 #define CU(call)                                             \

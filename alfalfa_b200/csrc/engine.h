@@ -122,8 +122,9 @@ struct TokJob {
 // stays free of CUDA includes.  Return 0 or a cudaError_t value.
 int launch_inter(const DevJob* jobs, int njobs, const Geom& g, void* stream);
 int launch_enc_rd_trellis(const EncJob* job, int rows, const Geom& g, int* ticket, void* stream);
-int launch_reenc_inter(const ReencJob* job, int n_mbs, const Geom& g, void* stream);
-int launch_reenc_intra(const ReencJob* job, int rows, const Geom& g, int* ticket, void* stream);
+// re-encoding: njobs frames of the context in one launch (each job its own target, records, tokens and counters)
+int launch_reenc_inter(const ReencJob* jobs, int njobs, int n_mbs, const Geom& g, void* stream);
+int launch_reenc_intra(const ReencJob* jobs, int njobs, int rows, const Geom& g, int* ticket, void* stream);
 // `epoch`: a value no earlier launch on this context has used (Engine::next_epoch); it marks the hand-over
 // messages of this launch.  epoch == 0 selects the round-1 kernels (progress counters + acquire / release).
 int launch_intra(const DevJob* jobs, int njobs, const Geom& g, int* ticket, uint32_t epoch, void* stream);

@@ -146,6 +146,9 @@ class Engine {
   const char* last_error() const { return err_.c_str(); }
   int fail(int code, const std::string& what);
   int cuda_fail(cudaError_t e, const char* what);
+  // the message of the calling thread's last fail / cuda_fail (of any Engine): work spread over host threads tells its
+  // own failures apart from the other threads' (last_error is the context's, whichever thread wrote it last)
+  static std::string& thread_error();
 
  private:
   Engine() = default;

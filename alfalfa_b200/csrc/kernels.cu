@@ -2307,12 +2307,13 @@ int launch_enc_rd_trellis(const EncJob* job, int rows, const Geom& g, int* ticke
   return (int)cudaGetLastError();
 }
 
-int launch_reenc_inter(const ReencJob* job, int n_mbs, const Geom& g, void* stream) {
-  VP8_LAUNCH(k_reenc_inter, (n_mbs + REENC_WARPS - 1) / REENC_WARPS, 32 * REENC_WARPS, 0, static_cast<cudaStream_t>(stream))(job, g);
+int launch_reenc_inter(const ReencJob* jobs, int njobs, int n_mbs, const Geom& g, void* stream) {
+  const dim3 grid((n_mbs + REENC_WARPS - 1) / REENC_WARPS, njobs);
+  VP8_LAUNCH(k_reenc_inter, grid, 32 * REENC_WARPS, 0, static_cast<cudaStream_t>(stream))(jobs, njobs, g);
   return (int)cudaGetLastError();
 }
-int launch_reenc_intra(const ReencJob* job, int rows, const Geom& g, int* ticket, void* stream) {
-  VP8_LAUNCH(k_reenc_intra, (rows + WF_WARPS - 1) / WF_WARPS, 32 * WF_WARPS, 0, static_cast<cudaStream_t>(stream))(job, g, ticket);
+int launch_reenc_intra(const ReencJob* jobs, int njobs, int rows, const Geom& g, int* ticket, void* stream) {
+  VP8_LAUNCH(k_reenc_intra, (njobs * rows + WF_WARPS - 1) / WF_WARPS, 32 * WF_WARPS, 0, static_cast<cudaStream_t>(stream))(jobs, njobs, g, ticket);
   return (int)cudaGetLastError();
 }
 

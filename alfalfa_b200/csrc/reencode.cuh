@@ -115,10 +115,11 @@ struct __align__(16) ReencInterSmem {  // per warp
   int16_t coef[COEF_I16];
 };
 
-// step 2: tokens of every inter macroblock.  J.recon holds the predictions (step 1).
-__global__ void __launch_bounds__(32 * REENC_WARPS) k_reenc_inter(const ReencJob* __restrict__ jobp, Geom g) {
+// step 2: tokens of every inter macroblock.  J.recon holds the predictions (step 1).  One launch serves njobs frames
+// of the context (Encoder::update_residues of several Encoders at once): job blockIdx.y, macroblocks along blockIdx.x.
+__global__ void __launch_bounds__(32 * REENC_WARPS) k_reenc_inter(const ReencJob* __restrict__ jobp, int njobs, Geom g) {
   __shared__ ReencInterSmem s_all[REENC_WARPS];
-  const ReencJob& J = *jobp;
+  const ReencJob& J = jobp[blockIdx.y];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int mbi = blockIdx.x * REENC_WARPS + warp;
   if (mbi >= J.cols * J.rows) return;
@@ -154,10 +155,9 @@ __global__ void __launch_bounds__(32 * REENC_WARPS) k_reenc_inter(const ReencJob
 }
 
 // step 4: the intra macroblocks, in dependency order.  J.recon holds every inter macroblock reconstructed (step 3).
-__global__ void __launch_bounds__(32 * WF_WARPS, 8) k_reenc_intra(const ReencJob* __restrict__ jobp, Geom g, int* ticket) {
+__global__ void __launch_bounds__(32 * WF_WARPS, 8) k_reenc_intra(const ReencJob* __restrict__ jobp, int njobs, Geom g, int* ticket) {
   __shared__ EncSmem s_all[WF_WARPS];
   __shared__ uint16_t s_lut[128];
-  const ReencJob& J = *jobp;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   for (int i = threadIdx.x; i < 128; i += blockDim.x) s_lut[i] = k_bpred_lut[i];
   __syncthreads();
@@ -170,7 +170,10 @@ __global__ void __launch_bounds__(32 * WF_WARPS, 8) k_reenc_intra(const ReencJob
   int t = 0;
   if (lane == 0) t = atomicAdd(ticket, 1);
   t = __shfl_sync(0xffffffffu, t, 0);
-  const int row = t;
+  // ticket t -> row t / njobs of job t % njobs (as k_enc_rd): the row a warp waits for, row - 1 of the same job, holds
+  // ticket t - njobs, so it was claimed by a warp that is already running; every job has its own progress counters
+  const ReencJob& J = jobp[t % njobs];
+  const int row = t / njobs;
   const int cols = J.cols, rows = J.rows;
   if (row >= rows) return;
   int* progress = J.progress + row;

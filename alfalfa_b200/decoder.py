@@ -507,38 +507,44 @@ class Encoder:
             raise RuntimeError("prediction/original_rasters mismatch")
         out = []
         start = 1 if extra_frame_chunk else 0
-
-        def qi_of(f):
-            q = self.L.vp8gpu_parsed_y_ac_qi(f.h)
-            if q < 0:
-                raise capi.LogicError(capi.ERR_LOGIC, "reencode: prediction frames must be parsed with keep_labels")
-            return q
-
-        def lrint(x):  # round half to even, like lrint in the default rounding mode
-            return int(round(x))
-
         for i in range(start, len(original_rasters)):
             y, u, v = original_rasters[i]
             pred = prediction_frames[i]
-            last = i == len(prediction_frames) - 1
-            is_key = bool(pred.desc.key_frame)
-            if i == start and is_key:
-                # option 1: an initial key frame becomes an inter frame (reencode_as_interframe, reencode.cc:39-129)
-                qi = qi_of(pred)
-                if i + 1 < len(prediction_frames) and not prediction_frames[i + 1].desc.key_frame:
-                    qi = lrint(kf_q_weight * qi_of(pred) + (1 - kf_q_weight) * qi_of(prediction_frames[i + 1]))
+            kind, qi, last = _reencode_step(self.L, i, prediction_frames, kf_q_weight, extra_frame_chunk)
+            if kind == "interframe":
                 out.append(self.reencode_as_interframe(y, u, v, pred, qi))
-            elif i == start and extra_frame_chunk:
-                # option 2: first inter frame of an extra-frame chunk: blend in the key frame's quantiser
-                if not prediction_frames[0].desc.key_frame:
-                    raise RuntimeError("extra-frame chunks must start with a keyframe.")
-                qi = lrint(kf_q_weight * qi_of(prediction_frames[0]) + (1 - kf_q_weight) * qi_of(pred))
-                out.append(self.update_residues(y, u, v, pred, qi, last))
-            elif is_key:
-                out.append(self.write_frame(pred))      # option 3: another key frame is preserved
+            elif kind == "write":
+                out.append(self.write_frame(pred))
             else:
-                out.append(self.update_residues(y, u, v, pred, -1, last))  # option 4
+                out.append(self.update_residues(y, u, v, pred, qi, last))
         return out
+
+    @staticmethod
+    def update_residues_batch(jobs):
+        """update_residues of several Encoders of one context in one set of kernel launches (vp8gpu_encoder_update_residues_batch).
+        jobs: (encoder, y, u, v, prediction_frame[, y_ac_qi[, last_frame]]) tuples, one per Encoder.  Every job runs (a refused
+        one leaves its Encoder unchanged); raises for the first failed job afterwards.  Returns the emitted frame of each job,
+        the same bytes as its encoder.update_residues would have returned."""
+        if not jobs:
+            return []
+        arr = (capi.ReencodeJob * len(jobs))()
+        keep = []
+        for j, job in zip(arr, jobs):
+            enc, y, u, v, pred = job[:5]
+            y_ac_qi = job[5] if len(job) > 5 else -1
+            last_frame = job[6] if len(job) > 6 else False
+            y, u, v = enc._planes(y, u, v)
+            keep.append((y, u, v))
+            j.encoder, j.y, j.u, j.v = enc.h.value, y.ctypes.data, u.ctypes.data, v.ctypes.data
+            j.y_stride, j.uv_stride = y.shape[1], u.shape[1]
+            j.prediction_frame, j.y_ac_qi, j.last_frame = pred.h.value, int(y_ac_qi), int(bool(last_frame))
+            j.out, j.cap = enc._out.ctypes.data, enc._out.size
+        ctx = jobs[0][0].ctx
+        rc = ctx.L.vp8gpu_encoder_update_residues_batch(arr, len(jobs))
+        if rc != capi.OK:  # the context's last error names the first failed job and its own failure
+            failed = [j.status for j in arr if j.status != capi.OK]
+            check(failed[0] if failed else rc, ctx.h, "update_residues_batch")
+        return [enc._out[:j.size].tobytes() for (enc, *_), j in zip(jobs, arr)]
 
     def reencode_as_interframe(self, y, u, v, key_frame, y_ac_qi):
         """Encoder::reencode_as_interframe (encoder/reencode.cc:39-129)"""
@@ -568,6 +574,73 @@ class Encoder:
         fid = C.c_int32(-1)
         check(self.L.vp8gpu_encoder_reconstruction(self.h, C.byref(fid)), self.ctx.h, "encoder_reconstruction")
         return RasterHandle(self.ctx, fid.value)
+
+
+def _reencode_step(L, i, prediction_frames, kf_q_weight, extra_frame_chunk):
+    """What Encoder::reencode (encoder/reencode.cc:315-381) does with frame i of a chunk: ("interframe", y_ac_qi, _),
+    ("write", _, _) or ("residues", y_ac_qi, last_frame)"""
+    def qi_of(f):
+        q = L.vp8gpu_parsed_y_ac_qi(f.h)
+        if q < 0:
+            raise capi.LogicError(capi.ERR_LOGIC, "reencode: prediction frames must be parsed with keep_labels")
+        return q
+
+    def lrint(x):  # round half to even, like lrint in the default rounding mode
+        return int(round(x))
+
+    start = 1 if extra_frame_chunk else 0
+    pred = prediction_frames[i]
+    last = i == len(prediction_frames) - 1
+    is_key = bool(pred.desc.key_frame)
+    if i == start and is_key:
+        # option 1: an initial key frame becomes an inter frame (reencode_as_interframe, reencode.cc:39-129)
+        qi = qi_of(pred)
+        if i + 1 < len(prediction_frames) and not prediction_frames[i + 1].desc.key_frame:
+            qi = lrint(kf_q_weight * qi_of(pred) + (1 - kf_q_weight) * qi_of(prediction_frames[i + 1]))
+        return "interframe", qi, last
+    if i == start and extra_frame_chunk:
+        # option 2: first inter frame of an extra-frame chunk: blend in the key frame's quantiser
+        if not prediction_frames[0].desc.key_frame:
+            raise RuntimeError("extra-frame chunks must start with a keyframe.")
+        return "residues", lrint(kf_q_weight * qi_of(prediction_frames[0]) + (1 - kf_q_weight) * qi_of(pred)), last
+    if is_key:
+        return "write", -1, last  # option 3: another key frame is preserved
+    return "residues", -1, last  # option 4
+
+
+def reencode_chunks(encoders, original_rasters_per_chunk, prediction_frames_per_chunk, kf_q_weight=1.0, extra_frame_chunk=False):
+    """Encoder::reencode of many independent chunks at once: chunk c is re-encoded by encoders[c] (distinct Encoders of
+    one context) and the result for each chunk is exactly what encoders[c].reencode(...) returns for it alone.  The
+    driver walks frame positions: the update_residues frames (options 2 and 4) of every chunk at a position go through
+    one Encoder.update_residues_batch; reencode_as_interframe (option 1) and write_frame (option 3) keep their single
+    calls; shorter chunks drop out when they end.  Returns the list of emitted frames of every chunk."""
+    if not (len(encoders) == len(original_rasters_per_chunk) == len(prediction_frames_per_chunk)):
+        raise RuntimeError("one Encoder, one list of rasters and one list of prediction frames per chunk")
+    for rasters, preds in zip(original_rasters_per_chunk, prediction_frames_per_chunk):
+        if not rasters:
+            raise RuntimeError("no rasters to re-encode")
+        if len(rasters) != len(preds):
+            raise RuntimeError("prediction/original_rasters mismatch")
+    outs = [[] for _ in encoders]
+    start = 1 if extra_frame_chunk else 0
+    longest = max((len(r) for r in original_rasters_per_chunk), default=0)
+    for i in range(start, longest):
+        batch = []
+        for c, (enc, rasters, preds) in enumerate(zip(encoders, original_rasters_per_chunk, prediction_frames_per_chunk)):
+            if i >= len(rasters):
+                continue
+            y, u, v = rasters[i]
+            kind, qi, last = _reencode_step(enc.L, i, preds, kf_q_weight, extra_frame_chunk)
+            if kind == "interframe":
+                outs[c].append(enc.reencode_as_interframe(y, u, v, preds[i], qi))
+            elif kind == "write":
+                outs[c].append(enc.write_frame(preds[i]))
+            else:
+                batch.append((c, (enc, y, u, v, preds[i], qi, last)))
+        if batch:
+            for (c, _), f in zip(batch, Encoder.update_residues_batch([job for _, job in batch])):
+                outs[c].append(f)
+    return outs
 
 
 def write_ivf(width, height, frames, expected_decoder_minihash=0):

@@ -259,7 +259,19 @@ struct SourceFrame {
   size_t y_stride, uv_stride;
 };
 
+class Encoder;
+// one job of update_residues_batch: as encoder->update_residues(target, *prediction_frame, y_ac_qi, last_frame)
+struct ReencodeJob {
+  Encoder* encoder;
+  SourceFrame target;
+  const ParsedFrame* prediction_frame;
+  int y_ac_qi;
+  bool last_frame;
+};
+inline std::vector<std::vector<uint8_t>> update_residues_batch(const std::vector<ReencodeJob>& jobs);
+
 class Encoder {
+  friend std::vector<std::vector<uint8_t>> update_residues_batch(const std::vector<ReencodeJob>& jobs);
   Context ctx_;
   uint16_t width_, height_;
   vp8gpu_encoder* h_ = nullptr;
@@ -410,5 +422,34 @@ class Encoder {
     return RasterHandle(ctx_, id);
   }
 };
+
+// update_residues of several Encoders of one context (each at most once) in one set of kernel launches
+// (vp8gpu_encoder_update_residues_batch): ExCamera's chunks are independent, so the frames at one position of many
+// chunks are re-encoded together.  Job i emits exactly what jobs[i].encoder->update_residues(...) would; every job runs,
+// a refused one leaves its Encoder unchanged, and the first failed job's error is thrown afterwards.
+inline std::vector<std::vector<uint8_t>> update_residues_batch(const std::vector<ReencodeJob>& jobs) {
+  std::vector<vp8gpu_reencode_job> c(jobs.size());
+  for (size_t i = 0; i < jobs.size(); i++) {
+    const ReencodeJob& j = jobs[i];
+    vp8gpu_reencode_job& r = c[i];
+    r = vp8gpu_reencode_job();
+    r.encoder = j.encoder->h_;
+    r.y = j.target.y, r.u = j.target.u, r.v = j.target.v, r.y_stride = j.target.y_stride, r.uv_stride = j.target.uv_stride;
+    r.prediction_frame = j.prediction_frame->get();
+    r.y_ac_qi = j.y_ac_qi, r.last_frame = j.last_frame;
+    r.out = j.encoder->buf_.data(), r.cap = j.encoder->buf_.size();
+  }
+  if (jobs.empty()) return {};
+  int rc = vp8gpu_encoder_update_residues_batch(c.data(), (int)c.size());
+  for (const vp8gpu_reencode_job& r : c)  // the first failed job's class; the context's last error names that job
+    if (rc != VP8GPU_OK && r.status != VP8GPU_OK) {
+      rc = r.status;
+      break;
+    }
+  check(rc, jobs[0].encoder->ctx_.get(), "update_residues_batch");
+  std::vector<std::vector<uint8_t>> out;
+  for (size_t i = 0; i < jobs.size(); i++) out.push_back(jobs[i].encoder->take(c[i].size));
+  return out;
+}
 
 }  // namespace alfalfa_gpu

@@ -465,6 +465,33 @@ int vp8gpu_encoder_estimate_frame_size(vp8gpu_encoder* enc, const uint8_t* y, si
 int vp8gpu_encoder_update_residues(vp8gpu_encoder* enc, const uint8_t* y, size_t y_stride, const uint8_t* u,
                                    const uint8_t* v, size_t uv_stride, const vp8gpu_parsed* prediction_frame, int y_ac_qi,
                                    int last_frame, uint8_t* out, size_t cap, size_t* size);
+/* update_residues of many chunks at once (ExCamera re-encodes its chunks independently of each other): one job per
+ * Encoder, all of them run through one set of kernel launches (prediction, residues, reconstruction, intra wavefront),
+ * one download, the frame writers on host threads and one set of decode launches that advances every Encoder.
+ *  - Each job behaves exactly as vp8gpu_encoder_update_residues on its encoder would: the same bytes, the same Encoder
+ *    state afterwards, the same refusals (y, u, v, prediction_frame, y_ac_qi, last_frame, out, cap, size as there).
+ *  - Jobs are independent: a refused job (VP8GPU_ERR_UNSUPPORTED for a segment-map update, VP8GPU_ERR_LOGIC for a key
+ *    frame, missing labels or a size mismatch, VP8GPU_ERR_NOMEM with `size` set for a too small `out`) gets its own
+ *    `status` and leaves its Encoder unchanged while the other jobs run.  A CUDA failure of a shared launch fails every
+ *    job in it, and none of those Encoders advance.
+ *  - VP8GPU_ERR_LOGIC for the whole call, no job run: the same Encoder twice (its frames depend on each other),
+ *    Encoders of different contexts, n < 0.
+ *  - Returns VP8GPU_OK when every job succeeded, otherwise the status of the first failed job; vp8gpu_last_error then
+ *    names that job and its own failure.
+ *  - vp8gpu_encoder_timeline of every Encoder that ran holds the batch's phases: [0] target uploads, [3] kernels +
+ *    download, [5] frame writers, [6] state update, [7] the whole call. */
+typedef struct vp8gpu_reencode_job {
+  vp8gpu_encoder* encoder;
+  const uint8_t *y, *u, *v; /* target, display size */
+  size_t y_stride, uv_stride;
+  const vp8gpu_parsed* prediction_frame; /* parsed with vp8gpu_parsed_keep_labels */
+  int y_ac_qi, last_frame;               /* as vp8gpu_encoder_update_residues */
+  uint8_t* out;
+  size_t cap;
+  size_t size; /* output: bytes of the emitted frame (also when `cap` was too small) */
+  int status;  /* output: VP8GPU_OK or the job's error */
+} vp8gpu_reencode_job;
+int vp8gpu_encoder_update_residues_batch(vp8gpu_reencode_job* jobs, int n);
 /* Encoder::reencode_as_interframe + write_frame (reencode.cc:39-129, 343-351): the chunk's initial key frame is coded
  * again as an inter frame predicted from this encoder's LAST (the reference's inter-frame decision loop on the
  * device), at the key frame's quantiser indices with y_ac_qi replaced, with its sharpness, refreshing all three
@@ -487,7 +514,8 @@ int vp8gpu_encoder_stats(const vp8gpu_encoder* enc, double* ssim, int* loop_filt
  * the search visited, [3] the full pass (decisions, transforms, reconstruction) incl. download of records and tokens,
  * [4] loop-filter search (the frame writer runs next to it), [5] the frame writer's own work (host thread, next to [4]; its wait for
  * the level is not counted), [6] state update (parse of the emitted frame's first partition, reference hand-over), [7] the whole
- * call.  n <= 8 values are written. */
+ * call.  After vp8gpu_encoder_update_residues_batch: [0] target uploads, [3] kernels + download, [5] writers, [6] state
+ * update, [7] the whole call, the other slots 0.  n <= 8 values are written. */
 int vp8gpu_encoder_timeline(const vp8gpu_encoder* enc, double* ms, int n);
 /* the reconstruction of the last encoded frame = the decoder's LAST reference after decoding it
  * (Encoder::export_decoder, encoder.hh:378); the caller releases the returned raster */
