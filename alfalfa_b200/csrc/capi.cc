@@ -996,7 +996,7 @@ struct IvfKnobs {
   int tok_arena = -1;      // VP8GPU_TOK_ARENA     token arena per worker, in largest frames (never below plan()'s floor)
   int dispatchers = -1;    // VP8GPU_DISPATCHERS   dispatcher threads
   int worker_nice = -1;    // VP8GPU_WORKER_NICE   niceness of the parsing workers (0 = leave alone)
-  bool trace = false;      // VP8GPU_TRACE         per-batch device times and per-worker arena counters on stderr
+  bool trace = false;      // VP8GPU_TRACE         per-batch device times, per-worker arena counters and chunk latencies on stderr
   bool parse_cache = false;  // VP8GPU_PARSE_CACHE  diagnostic: replay remembered first partitions (see above)
   static int num(const char* name) {
     const char* v = getenv(name);
@@ -1144,7 +1144,7 @@ void IvfDecode::plan() {
   // device-side token decoding needs rasters for the frames a worker keeps in flight
   if (ctx->device_tokens.load()) {
     tok_slots = e->frames_free() / threads - 4;
-    // k_tokens needs tens of milliseconds per frame (one thread each), so a worker wants to run a
+    // k_tokens needs 20-105 ms per 1080p frame (one thread each; H100, bench GOPs), so a worker wants to run a
     // GOP or two ahead of the pixel kernels; bounded by a device-memory budget for the rings: half of the
     // device (40 GB of an 80 GB H100), the other half for the rasters of the workers' frames in flight.
     // Measured on an H100 (bench.py 1080p, 64 workers): a quarter of the device leaves fewer slots per worker
@@ -1381,6 +1381,12 @@ void IvfDecode::worker_device(int tid) {
   size_t head = 0, a_start[kTokSlots] = {};
   bool held[kTokSlots] = {};
   long n_takes = 0, n_wraps = 0, n_waits = 0;
+  // VP8GPU_TRACE: per chunk, timing events at "staged" (copy stream), "k_tokens may start" and "ready" (kernel stream)
+  struct ChunkTrace {
+    cudaEvent_t ev[3];
+    int frames;
+  };
+  std::vector<ChunkTrace> chunk_trace;
   auto arena_take = [&](int si, size_t need, auto in_chunk, vp8gpu_token** out) {
     const size_t cap = arena_tokens;
     if (held[si]) {  // the slot's previous frame is done: its space is the oldest
@@ -1475,6 +1481,12 @@ void IvfDecode::worker_device(int tid) {
       kit->next_kstream = (kit->next_kstream + 1) % kTokStreams;
       cudaEventRecord(kit->staged[first_slot], kit->copy_stream);
       cudaStreamWaitEvent(ks, kit->staged[first_slot], 0);
+      ChunkTrace ctr{{nullptr, nullptr, nullptr}, staged};
+      if (knobs.trace) {
+        for (cudaEvent_t& ev : ctr.ev) cudaEventCreate(&ev);
+        cudaEventRecord(ctr.ev[0], kit->copy_stream);
+        cudaEventRecord(ctr.ev[1], ks);
+      }
       if (ctx->tok_capacity > 0) {  // permits for the frames of this launch (returned by tok_release_cb when the kernel is done)
         std::unique_lock<std::mutex> lk(ctx->tok_mu);
         const int need = staged < ctx->tok_capacity ? staged : ctx->tok_capacity;
@@ -1488,6 +1500,10 @@ void IvfDecode::worker_device(int tid) {
       if (rc == VP8GPU_OK && staged > until_wrap) rc = e->token_ring_launch(kit->ring, 0, staged - until_wrap, ks);
       if (rc == VP8GPU_OK)
         cudaEventRecord(kit->ready[first_slot], ks);  // one event per launch: its frames become ready together
+      if (knobs.trace) {
+        cudaEventRecord(ctr.ev[2], ks);
+        chunk_trace.push_back(ctr);
+      }
       // the permits come back when the stream gets here (also after a failed launch); queued after the
       // `ready` events so that the host-function thread is not on the frames' critical path
       if (permits_taken && cudaLaunchHostFunc(ks, tok_release_cb, new TokRelease{ctx, permits_taken}) != cudaSuccess) {
@@ -1570,9 +1586,28 @@ void IvfDecode::worker_device(int tid) {
         }
       if (cleared) cudaStreamSynchronize(kit->copy_stream);
     }
-    if (knobs.trace)
+    if (knobs.trace) {
       fprintf(stderr, "decode_ivf arena: worker %d takes %ld wraps %ld waits %ld cap %zu slots %d chunk %d\n", tid, n_takes, n_wraps,
               n_waits, arena_tokens, tok_slots, tok_chunk);
+      // chunk latency: staged -> ready (what a dispatcher waits for) and k_tokens start -> ready (the kernel, residency included)
+      std::vector<float> lat, kern;
+      long frames = 0;
+      for (ChunkTrace& c : chunk_trace) {
+        float ms = 0;
+        if (cudaEventElapsedTime(&ms, c.ev[0], c.ev[2]) == cudaSuccess) lat.push_back(ms);
+        if (cudaEventElapsedTime(&ms, c.ev[1], c.ev[2]) == cudaSuccess) kern.push_back(ms);
+        frames += c.frames;
+        for (cudaEvent_t ev : c.ev) cudaEventDestroy(ev);
+      }
+      auto pct = [](std::vector<float>& v, double q) {
+        if (v.empty()) return 0.0;
+        std::sort(v.begin(), v.end());
+        return (double)v[std::min(v.size() - 1, (size_t)(q * (v.size() - 1) + 0.5))];
+      };
+      fprintf(stderr, "[trace] worker %d chunks: %zu (%ld frames); staged -> ready ms p10 %.2f p50 %.2f p90 %.2f max %.2f; "
+              "k_tokens start -> ready ms p50 %.2f p90 %.2f max %.2f\n", tid, chunk_trace.size(), frames, pct(lat, 0.1), pct(lat, 0.5),
+              pct(lat, 0.9), pct(lat, 1.0), pct(kern, 0.5), pct(kern, 0.9), pct(kern, 1.0));
+    }
     std::lock_guard<std::mutex> lk(ctx->pool_mu);
     ctx->kit_pool.push_back(kit);
   }

@@ -1,7 +1,9 @@
 #!/usr/bin/env python3
 """GPU-box tool: sweep the host-side knobs of vp8gpu_decode_ivf on the bench workload (output left on the device)
-and print Mpix/s, the host time accounting and -- with VP8GPU_TRACE=1 -- the per-batch device times.
-usage: tools/e2e_probe.py [--configs "threads:dispatchers:nice,..."] [--steps N]"""
+and print Mpix/s, the host time accounting and -- with --trace (VP8GPU_TRACE=1) -- the per-batch device times of every
+dispatcher and, per worker, the distribution of its chunks' latency from "staged" to "ready" (k_tokens).
+The bench shape: --configs 64:4:5 --streams 258.
+usage: tools/e2e_probe.py [--configs "threads:dispatchers:nice,..."] [--steps N] [--trace]"""
 import argparse
 import ctypes as C
 import os
@@ -18,7 +20,10 @@ def main():
     ap.add_argument("--configs", default="64:4:5,64:4:0,64:2:5,64:1:5,64:8:5,32:2:5,128:4:5,128:8:5")
     ap.add_argument("--steps", type=int, default=2)
     ap.add_argument("--streams", type=int, default=258)
+    ap.add_argument("--trace", action="store_true", help="VP8GPU_TRACE=1: per-batch and per-chunk device times on stderr")
     a = ap.parse_args()
+    if a.trace:
+        os.environ["VP8GPU_TRACE"] = "1"
     import bench
     from alfalfa_b200 import Context, capi
     w, h, instances = bench.load_instances(bench.WORKLOADS["1080p"], per_clip=0)
