@@ -377,7 +377,7 @@ int filter_frame(vp8gpu_encoder* enc, int frame, bool key, int level) {
   CUE(cudaMemsetAsync(d_sync + 32, 0, sizeof(int), s));                                     // ticket
   CUE(cudaMemsetAsync(d_sync + 128 + g.mb_rows, 0, sizeof(int) * (size_t)g.mb_rows, s));    // row progress
   const vp8::DevJob* d_dj = reinterpret_cast<const vp8::DevJob*>(enc->dev + enc->off_encjob + 512);
-  if (int ce = vp8::launch_loopfilter(d_dj, 1, g, d_sync + 32, e->next_epoch(2), s)) return e->cuda_fail((cudaError_t)ce, "k_loopfilter");
+  if (int ce = vp8::launch_loopfilter(d_dj, 1, g, d_sync + 32, e->next_epoch(2), e->lf_band(), s)) return e->cuda_fail((cudaError_t)ce, "k_loopfilter");
   e->count_launches(1);
   e->mark_frames(enc->lane, ids, 1);
   // the pinned descriptor is rewritten by the next call: wait until it has been read
@@ -414,7 +414,7 @@ int filter_batch(vp8gpu_encoder* enc, const int* frames, const int* levels, int 
   CUE(cudaMemsetAsync(d_sync + 32, 0, sizeof(int), s));                                         // ticket
   CUE(cudaMemsetAsync(d_sync + 128 + g.mb_rows, 0, sizeof(int) * (size_t)n * g.mb_rows, s));    // row progress
   const vp8::DevJob* d_dj = reinterpret_cast<const vp8::DevJob*>(enc->dev + enc->off_encjob + 512);
-  if (int ce = vp8::launch_loopfilter(d_dj, n, g, d_sync + 32, e->next_epoch(2), s)) return e->cuda_fail((cudaError_t)ce, "k_loopfilter");
+  if (int ce = vp8::launch_loopfilter(d_dj, n, g, d_sync + 32, e->next_epoch(2), e->lf_band(), s)) return e->cuda_fail((cudaError_t)ce, "k_loopfilter");
   e->count_launches(1);
   e->mark_frames(enc->lane, frames, n);
   // the pinned descriptors are rewritten by the next call: wait until they have been read

@@ -567,7 +567,7 @@ int Engine::build_and_launch(int lane, const DevJob* d_jobs, int* d_sync, int n,
   }
   if (between) CU(cudaEventRecord(between[1], s));
   if (any_lf) {
-    if (int e = launch_loopfilter(d_jobs, n, g_, d_sync + 32, next_epoch(2), s)) return cuda_fail((cudaError_t)e, "k_loopfilter launch");
+    if (int e = launch_loopfilter(d_jobs, n, g_, d_sync + 32, next_epoch(2), lf_band(), s)) return cuda_fail((cudaError_t)e, "k_loopfilter launch");
     launches_++;
   }
   return VP8GPU_OK;

@@ -126,9 +126,10 @@ int launch_enc_rd_trellis(const EncJob* job, int rows, const Geom& g, int* ticke
 int launch_reenc_inter(const ReencJob* jobs, int njobs, int n_mbs, const Geom& g, void* stream);
 int launch_reenc_intra(const ReencJob* jobs, int njobs, int rows, const Geom& g, int* ticket, void* stream);
 // `epoch`: a value no earlier launch on this context has used (Engine::next_epoch); it marks the hand-over
-// messages of this launch.  epoch == 0 selects the round-1 kernels (progress counters + acquire / release).
+// messages of this launch.  epoch == 0 selects the round-1 kernels (progress counters + acquire / release);
+// for the loop filter `band` then selects k_loopfilter_band (rows hand over inside a CTA) over k_loopfilter.
 int launch_intra(const DevJob* jobs, int njobs, const Geom& g, int* ticket, uint32_t epoch, void* stream);
-int launch_loopfilter(const DevJob* jobs, int njobs, const Geom& g, int* ticket, uint32_t epoch, void* stream);
+int launch_loopfilter(const DevJob* jobs, int njobs, const Geom& g, int* ticket, uint32_t epoch, bool band, void* stream);
 // token jobs sit at the start of equally spaced ring slots: slot (first + i) % nslots for block i
 int launch_tokens(const uint8_t* ring, size_t stride, int first, int count, int nslots, const Geom& g, void* stream);
 int launch_fetch_header(void* dst, const void* src_host_devptr, size_t bytes, void* stream);  // bytes % 16 == 0

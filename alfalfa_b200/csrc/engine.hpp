@@ -83,6 +83,7 @@ class Engine {
     if (e == 0) e = ++epoch_;
     return e;
   }
+  bool lf_band() const { return ll_mask_ & 4; }
   int frame_upload(int id, const uint8_t* y, size_t ys, const uint8_t* u, const uint8_t* v, size_t cs);
   int frame_download(int id, uint8_t* y, size_t ys, uint8_t* u, uint8_t* v, size_t cs);
   int frame_download_display(int id, int lane, uint8_t* dst, size_t dst_size, bool wait);
@@ -200,8 +201,10 @@ class Engine {
   std::mutex err_mu_;
   std::atomic<uint32_t> epoch_{0};
   // which wavefront kernels use hand-over messages (bit 0 intra prediction, bit 1 loop filter); the others run
-  // the round-1 kernels (progress counters).  VP8GPU_WAVEFRONT = legacy | ll | intra-ll | lf-ll for A/B runs.
-  int ll_mask_ = 1;
+  // the round-1 kernels (progress counters).  Bit 2: the loop filter without messages is k_loopfilter_band
+  // (bands of rows per CTA) rather than k_loopfilter.  VP8GPU_WAVEFRONT = legacy | ll | intra-ll | lf-ll selects
+  // the earlier kernel pairs for A/B runs.
+  int ll_mask_ = 1 | 4;
 };
 
 }  // namespace vp8

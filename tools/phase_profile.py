@@ -1,7 +1,8 @@
 #!/usr/bin/env python3
 """GPU-box tool: where does a macroblock step of the wavefront kernels spend its cycles?
 Uses the -DVP8_PROFILE build of the library (alfalfa_b200/csrc/build.sh prof), decodes frames of the
-bench clip through the HBM-resident batch API and prints average clock64() cycles per phase per MB.
+bench clip through the HBM-resident batch API and prints average clock64() cycles per phase per MB.  The loop filter's
+phases are k_loopfilter_band's (the default) unless VP8GPU_WAVEFRONT selects another kernel pair.
 usage: tools/phase_profile.py [--g N]"""
 import argparse
 import ctypes as C
@@ -19,12 +20,15 @@ from alfalfa_b200 import Context, capi  # noqa: E402
 
 INTRA = ["load_mb", "build_residuals", "wait_row", "edge loads", "predict+add", "store+next", "publish", "loop overhead"]
 LF = ["load_mb", "wait_row", "top/left loads+smem", "filter", "write back", "publish", "-", "loop overhead"]
+LF_BAND = ["load_mb", "wait in band", "wait between bands", "top/left loads+smem", "filter", "ring back-pressure",
+           "write back+publish", "loop overhead"]
 
 
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--g", type=int, default=1)
     a = ap.parse_args()
+    lf_labels = LF if os.environ.get("VP8GPU_WAVEFRONT") in ("legacy", "ll", "intra-ll", "lf-ll") else LF_BAND
     L = capi.lib()
     prof = C.CDLL(os.environ["VP8GPU_LIB"]).vp8gpu_debug_profile
     data = open(os.path.join(ROOT, "bench_data", "synth1080p_medium_q90.ivf"), "rb").read()
@@ -63,7 +67,7 @@ def main():
         print("frame %d (%s) x%d: k_inter %.3f ms  k_intra %.3f ms  k_loopfilter %.3f ms | intra MBs %d bpred %d filtered %d"
               % (30 + fi, "key" if d.key_frame else "inter", a.g, ms3[0], ms3[1], ms3[2], n_intra,
                  int((mbs["y_mode"] == 4).sum()), int((mbs["lf_level"] > 0).sum())))
-        for name, base, labels in (("k_intra", 0, INTRA), ("k_loopfilter", 16, LF)):
+        for name, base, labels in (("k_intra", 0, INTRA), ("k_loopfilter", 16, lf_labels)):
             n = v[base + 8]
             if not n:
                 continue
