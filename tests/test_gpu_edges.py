@@ -27,9 +27,10 @@ def _stream(name):
     return _cache[name]
 
 
-# unset = the default (intra-ll: k_intra_ll + k_loopfilter); legacy = k_intra with progress counters + k_loopfilter;
-# ll = k_intra_ll + k_loopfilter_ll; lf-ll = k_intra + k_loopfilter_ll (engine.cu reads it at every context creation)
-@pytest.fixture(params=[None, "legacy", "ll", "lf-ll"], ids=["default", "legacy", "ll", "lf-ll"])
+# unset = the default (k_intra_ll + k_loopfilter_band); legacy = k_intra with progress counters + k_loopfilter;
+# intra-ll = k_intra_ll + k_loopfilter; ll = k_intra_ll + k_loopfilter_ll; lf-ll = k_intra + k_loopfilter_ll
+# (engine.cu reads it at every context creation)
+@pytest.fixture(params=[None, "legacy", "intra-ll", "ll", "lf-ll"], ids=["default", "legacy", "intra-ll", "ll", "lf-ll"])
 def wavefront(request, monkeypatch):
     if request.param is None:
         monkeypatch.delenv("VP8GPU_WAVEFRONT", raising=False)

@@ -102,6 +102,15 @@ def test_edge_streams_emulated_in_both_thread_orders(simt_lib):
     run_gpu_tests_emulated(simt_lib, ["tests/test_gpu_edges.py"], env_extra={"SIMT_ORDER": "reverse"})
 
 
+def test_loopfilter_maps_emulated_in_both_thread_orders(simt_lib):
+    """tests/test_gpu_loopfilter.py (designed level maps under every loop-filter kernel) in the default thread order
+    and with SIMT_ORDER=reverse, where the last warp of a band runs first and spins on the ring flags; the 1024-column
+    and 1080p cases stay on the GPU"""
+    args = ["tests/test_gpu_loopfilter.py", "-k", "not 1024x and not bench"]
+    run_gpu_tests_emulated(simt_lib, args)
+    run_gpu_tests_emulated(simt_lib, args, env_extra={"SIMT_ORDER": "reverse"})
+
+
 def test_reencode_edges_emulated_in_both_thread_orders(simt_lib):
     """tests/test_gpu_reencode_edges.py (re-encoding at degenerate shapes, plane-edge windows and saturated targets)
     in the default thread order and with SIMT_ORDER=reverse; the 1080p and 16383-pixel-wide cases stay on the GPU"""
