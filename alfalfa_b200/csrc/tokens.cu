@@ -33,7 +33,7 @@ __global__ void __launch_bounds__(32 * kTokWarps) k_tokens(const uint8_t* ring, 
                                                           int nslots, Geom g) {
   __shared__ __align__(16) uint8_t probs_all[kTokWarps][tok::kProbBytes];
   __shared__ uint16_t above_all[kTokWarps][kMaxCols];
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int warp = kTokWarps == 1 ? 0 : threadIdx.x >> 5, lane = threadIdx.x & 31;  // a constant table address for one warp
   const int job = blockIdx.x * kTokWarps + warp;
   if (job >= count) return;
   uint8_t* probs = probs_all[warp];

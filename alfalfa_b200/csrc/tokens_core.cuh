@@ -55,20 +55,25 @@ TK_DEV void expand_prob_entry(const uint8_t* src, uint8_t* dst, int e) {
 // Bit-for-bit the decisions of csrc/parser.cc's BoolReader (and therefore bool_decoder.hh:82-107): past
 // the end of the partition only zero bits arrive.  A decode never waits for memory: the stream is fetched
 // as aligned 32-bit words ONE REFILL AHEAD (`nxt` is requested when the previous word is consumed, ~30
-// decisions before it is needed).  The 64-bit window is consumed from the top and holds `nbits` valid
-// bits.  Plain struct, always handled by value / reference to a local: stays in registers.
+// decisions before it is needed).  The window is 64 bits, consumed from the top, with `nbits` valid bits
+// (the rest zero); it is kept as two words, `hi` and `lo`, because a decision compares and subtracts in
+// `hi` alone and normalising is one funnel shift of (hi, lo).  The range is kept as range << 16, so that
+// one multiply-add gives the split already in the top byte (lr_decide).  Plain struct, always handled by
+// value / reference to a local: stays in registers.
 #ifdef __CUDACC__
 #define TK_BSWAP(x) __byte_perm((x), 0, 0x0123)
+#define TK_FUNNEL_L(lo, hi, s) __funnelshift_l((lo), (hi), (s))
 #else
 #define TK_BSWAP(x) __builtin_bswap32(x)
+#define TK_FUNNEL_L(lo, hi, s) static_cast<uint32_t>(((static_cast<uint64_t>(hi) << 32) | (lo)) << (s) >> 32)
 #endif
 struct LaneReader {
   const uint8_t* p;    // next word to request (4-byte aligned)
   const uint8_t* end;
-  uint64_t value;
+  uint32_t hi, lo;     // the window: hi = its top 32 bits
   int nbits;
   uint32_t nxt;        // the next 32 bits of the stream, most significant bit first
-  uint32_t range;
+  uint32_t rng16;      // range << 16, range in [128, 255] between decisions
 };
 TK_DEV uint32_t lr_fetch(LaneReader& b) {
   uint32_t w = 0;
@@ -81,38 +86,58 @@ TK_DEV uint32_t lr_fetch(LaneReader& b) {
   b.p += 4;
   return w;
 }
-TK_DEV void lr_refill(LaneReader& b) {  // nbits <= 32 on entry
-  b.value |= static_cast<uint64_t>(b.nxt) << (32 - b.nbits);
+TK_DEV void lr_refill(LaneReader& b) {  // nbits <= 32 on entry, so lo == 0
+  const uint64_t v = (static_cast<uint64_t>(b.nxt) << 32) >> b.nbits;
+  b.hi |= static_cast<uint32_t>(v >> 32);
+  b.lo = static_cast<uint32_t>(v);
   b.nbits += 32;
   b.nxt = lr_fetch(b);
 }
 TK_DEV void lr_init(LaneReader& b, const uint8_t* data, uint32_t n) {
   b.p = data;
   b.end = data + n;
-  b.value = 0;
+  uint64_t value = 0;
   b.nbits = 0;
-  b.range = 255;
+  b.rng16 = 255u << 16;
   while ((reinterpret_cast<uintptr_t>(b.p) & 3) && b.p < b.end) {  // up to three bytes to reach a word boundary
-    b.value |= static_cast<uint64_t>(TK_LDG(b.p++)) << (56 - b.nbits);
+    value |= static_cast<uint64_t>(TK_LDG(b.p++)) << (56 - b.nbits);
     b.nbits += 8;
   }
+  b.hi = static_cast<uint32_t>(value >> 32);
+  b.lo = static_cast<uint32_t>(value);
   if (b.p >= b.end) b.p = reinterpret_cast<const uint8_t*>((reinterpret_cast<uintptr_t>(b.p) + 3) & ~static_cast<uintptr_t>(3));
   b.nxt = lr_fetch(b);
   lr_refill(b);
   if (b.nbits <= 32) lr_refill(b);
 }
 // One decision, without a refill test: the 8 compared bits must be valid (nbits >= 8), and the window
-// shifts by at most 7.  Only the high word of the window takes part in the compare.
+// shifts by at most 7.  With M = 0xFFFFFF and t = rng16 * prob + ((256 - prob) << 16), the top byte of t is
+// split = 1 + (((range - 1) * prob) >> 8) and t's low 24 bits are below 2^24, so
+//   hi >= split << 24          <=>  (hi | M) >= t
+//   (range - split) << 24      ==   ((rng16 << 8 | M) - t) & ~M
+// and what depends on the previous decision is a multiply-add, a compare, a select, FLO and a shift.  The low
+// 24 bits of the selected range do not change its leading zeros; they are dropped before it is shifted.
+#ifndef TK_ON_DECISION
+#define TK_ON_DECISION()  // host-only hook: tools/tokens_chain_count.cc counts decisions with it
+#endif
 TK_DEV int lr_decide(LaneReader& b, uint32_t prob) {
-  const uint32_t split = 1 + (((b.range - 1) * prob) >> 8);
-  uint32_t hi = static_cast<uint32_t>(b.value >> 32);
-  const uint32_t big = split << 24;
-  const int bit = hi >= big;
-  const uint32_t r = bit ? b.range - split : split;
-  hi -= bit ? big : 0u;
-  const int shift = TK_CLZ(r) - 24;
-  b.range = r << shift;
-  b.value = ((static_cast<uint64_t>(hi) << 32) | static_cast<uint32_t>(b.value)) << shift;
+  TK_ON_DECISION();
+  const uint32_t M = 0xFFFFFFu;
+  const uint32_t t = b.rng16 * prob + ((256u - prob) << 16);
+  const int bit = (b.hi | M) >= t;
+  const uint32_t r = bit ? ((b.rng16 << 8) | M) - t : t;  // (new range << 24) + bits below 2^24
+  const uint32_t h = bit ? b.hi - (t & ~M) : b.hi;
+#ifdef __CUDACC__
+  int shift;  // leading zeros of r (r != 0): FLO.SH gives them directly, __clz adds a subtraction from 31
+  asm("bfind.shiftamt.u32 %0, %1;" : "=r"(shift) : "r"(r));
+  const uint32_t r16 = __byte_perm(r, 0, 0x4344);  // (r >> 24) << 16
+#else
+  const int shift = TK_CLZ(r);
+  const uint32_t r16 = (r >> 24) << 16;
+#endif
+  b.rng16 = r16 << shift;
+  b.hi = TK_FUNNEL_L(b.lo, h, shift);
+  b.lo <<= shift;
   b.nbits -= shift;
   return bit;
 }
@@ -137,20 +162,43 @@ constexpr uint64_t kBandNibbles = 0x7666666665463210ull;  // c_band[i] = nibble 
 TK_DEV uint32_t band_off(int i) {  // byte offset of (band of position i & 15, ctx 0) in a block type's entries
   return static_cast<uint32_t>((kBandNibbles >> (4 * (i & 15))) & 15) * 48;
 }
-TK_DEV Probs16 ld_probs(const uint8_t* p) { return *reinterpret_cast<const Probs16*>(p); }
+// The probability table is addressed by its 32-bit shared-memory offset on the device (ProbAddr): the address
+// of an entry is then one integer add, not a generic pointer the compiler rebuilds from the CTA's shared
+// window (an S2R on the chain).  The load is volatile asm, so that it is issued where the source puts it --
+// ahead of the decision that selects its result -- and not sunk into the branch that uses it, where the next
+// decision would wait for it.
+#ifdef __CUDACC__
+typedef uint32_t ProbAddr;
+TK_DEV ProbAddr prob_addr(const uint8_t* p) {
+  // through an opaque move: the compiler would otherwise rebuild the address from SR_CgaCtaId at every use
+  uint32_t a;
+  asm volatile("mov.u32 %0, %1;" : "=r"(a) : "r"(static_cast<uint32_t>(__cvta_generic_to_shared(p))));
+  return a;
+}
+TK_DEV Probs16 ld_probs(ProbAddr a) {
+  Probs16 P;
+  asm volatile("ld.shared.v4.u32 {%0, %1, %2, %3}, [%4];"
+               : "=r"(P.w[0]), "=r"(P.w[1]), "=r"(P.w[2]), "=r"(P.w[3]) : "r"(a));
+  return P;
+}
+#else
+typedef const uint8_t* ProbAddr;
+TK_DEV ProbAddr prob_addr(const uint8_t* p) { return p; }
+TK_DEV Probs16 ld_probs(ProbAddr p) { return *reinterpret_cast<const Probs16*>(p); }
+#endif
 
 // One 4x4 block (tokens.cc:50-135).  tp = 16-byte probability entries of the block type,
 // i = first coefficient, tag = block number << 20.  Returns has_nonzero.
-TK_DEV int parse_block(LaneReader& br, const uint8_t* tp, int ctx, int i, uint32_t tag, vp8gpu_token*& out) {
+TK_DEV int parse_block(LaneReader& br, ProbAddr tp, int ctx, int i, uint32_t tag, vp8gpu_token*& out) {
   lr_ensure(br);
   Probs16 P = ld_probs(tp + band_off(i) + ctx * 16);
   if (!lr_decide(br, P.at(0))) return 0;
   int nz = 0;
   for (;;) {
     // group of decisions: p[1], p[2] and, for a ONE token, its sign and the next p[0]
-    lr_ensure(br);
     const uint32_t next = band_off(i + 1);      // position i + 1 (unused when i == 15)
     const Probs16 Pz = ld_probs(tp + next);      // its entry after a ZERO token (ctx 0)
+    lr_ensure(br);
     if (!lr_decide(br, P.at(1))) {  // zero token: no end-of-block test after a zero
       if (++i == 16) return nz;
       P = Pz;
@@ -214,10 +262,10 @@ TK_DEV void decode_frame_tokens(const TokJob& J, const Geom& g, const uint8_t* p
   vp8gpu_token* t = t_begin;
   const vp8gpu_token* const t_limit = t_begin + J.tok_cap;
   uint32_t overflow = 0;
-  const uint8_t* const coef_y_after_y2 = probs + 0 * 384;
-  const uint8_t* const coef_y2 = probs + 1 * 384;
-  const uint8_t* const coef_uv = probs + 2 * 384;
-  const uint8_t* const coef_y_full = probs + 3 * 384;
+  const ProbAddr coef_y_after_y2 = prob_addr(probs);
+  const ProbAddr coef_y2 = coef_y_after_y2 + 1 * 384;
+  const ProbAddr coef_uv = coef_y_after_y2 + 2 * 384;
+  const ProbAddr coef_y_full = coef_y_after_y2 + 3 * 384;
 
   // word 1 of a record = tok_cnt | y_mode << 16 | uv_mode << 24, word 2 = ref | segment | lf | flags << 24
   const uint32_t* rec = reinterpret_cast<const uint32_t*>(mbs);
@@ -248,7 +296,7 @@ TK_DEV void decode_frame_tokens(const TokJob& J, const Geom& g, const uint8_t* p
         a_nz = 0;
         left_nz = 0;
       } else {
-        const uint8_t* y_probs = coef_y_full;
+        ProbAddr y_probs = coef_y_full;
         int first = 0;
         if (has_y2) {
           const int ctx = ((a_nz >> 8) & 1) + ((left_nz >> 8) & 1);
@@ -262,7 +310,7 @@ TK_DEV void decode_frame_tokens(const TokJob& J, const Geom& g, const uint8_t* p
 #pragma unroll 1
         for (int b = 0; b < 24; b++) {
           int bx, by;
-          const uint8_t* tp;
+          ProbAddr tp;
           int f;
           if (b < 16) {
             bx = b & 3, by = b >> 2, tp = y_probs, f = first;
