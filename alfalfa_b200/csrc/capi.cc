@@ -95,7 +95,7 @@ struct ivf_worker_kit {
   cudaStream_t kstream[kTokStreams] = {};
   int next_kstream = 0;
   vp8gpu_parsed* parsed[kTokSlots] = {};
-  cudaEvent_t staged[kTokSlots] = {}, ready[kTokSlots] = {}, finished[kTokSlots] = {};
+  cudaEvent_t staged[kTokSlots] = {}, finished[kTokSlots] = {};
   bool busy[kTokSlots] = {};
 };
 struct vp8gpu_resident_batch {
@@ -175,7 +175,6 @@ void vp8gpu_ctx_destroy(vp8gpu_ctx* ctx) {
     for (int i = 0; i < kTokSlots; i++) {
       if (k->parsed[i]) vp8gpu_parsed_destroy(k->parsed[i]);
       if (k->staged[i]) cudaEventDestroy(k->staged[i]);
-      if (k->ready[i]) cudaEventDestroy(k->ready[i]);
     }
     delete k;
   }
@@ -1011,7 +1010,7 @@ struct IvfKnobs {
 // vp8gpu_decode_ivf as an object, one instance per call: parse_container() reads the IVF file into GOPs, plan() sizes
 // the pipeline (workers, token-ring slots, dispatchers), run() starts one thread per worker -- worker_host parses whole
 // frames, worker_device only first partitions and launches k_tokens for the rest -- and one per dispatcher, which
-// batches whatever the workers have queued (at most one frame per worker: consecutive frames of a GOP depend on each
+// batches whatever the workers have queued (at most one frame per GOP: consecutive frames of a GOP depend on each
 // other) onto the device.
 class IvfDecode {
  public:
@@ -1036,10 +1035,13 @@ class IvfDecode {
     int64_t out_off;
     int* slot_state;
     int tid = 0;  // the worker that queued it
-    // device-side tokens: the records live in ring slot `ring_slot` once `ready` has fired
+    int gop = 0;  // its GOP: a frame can go once the frame before it in its GOP has gone
+    // device-side tokens: the records live in ring slot `ring_slot` once k_tokens has published `epoch` to the slot's
+    // ready word in mapped host memory
     const vp8::TokenRing* ring = nullptr;
     int ring_slot = 0;
-    cudaEvent_t ready = nullptr;
+    const volatile uint32_t* ready_word = nullptr;
+    uint32_t epoch = 0;
     cudaEvent_t* finished = nullptr;  // where submit() leaves the event that fires after the pixel kernels
   };
 
@@ -1214,7 +1216,7 @@ void IvfDecode::plan() {
 }
 
 // Host workers only parse (CPU entropy front end) and keep the per-GOP codec state; a dispatcher gathers
-// whatever they have produced -- at most one frame per worker, because consecutive frames of a GOP depend on
+// whatever they have produced -- at most one frame per GOP, because consecutive frames of a GOP depend on
 // each other -- into ONE batched decode per round, so the device sees a few large launches instead of three small
 // ones per frame, and the wavefront kernels get rows of many frames to hide their latency with.
 void IvfDecode::worker_host(int tid) {
@@ -1283,6 +1285,7 @@ void IvfDecode::worker_host(int tid) {
         std::lock_guard<std::mutex> lk(mu);
         slot_state[si] = kQueued;
         job.tid = tid;
+        job.gop = g;
         queues[tid].push_back(job);
       }
       cv_disp[tid % n_disp].notify_one();
@@ -1324,7 +1327,7 @@ void IvfDecode::worker_host(int tid) {
 // ---- workers with device-side token decoding: the host only walks the first partition; the DCT
 //      partitions of up to tok_chunk frames go to the device in one k_tokens launch on the worker's
 //      own stream, tok_slots frames may be in flight per worker, and the dispatcher picks a frame up
-//      once its `ready` event has fired ----
+//      once k_tokens has published it (the slot's ready word), whatever the rest of its launch is doing ----
 ivf_worker_kit* IvfDecode::acquire_kit() {
   ivf_worker_kit* k = nullptr;
   {
@@ -1356,7 +1359,6 @@ ivf_worker_kit* IvfDecode::acquire_kit() {
     k->parsed[i]->f.mbs.reserve(n_mbs, 0);
     k->parsed[i]->f.split.reserve(256, 0);
     cudaEventCreateWithFlags(&k->staged[i], cudaEventDisableTiming);
-    cudaEventCreateWithFlags(&k->ready[i], cudaEventDisableTiming);
   }
   return k;
 }
@@ -1369,7 +1371,6 @@ void IvfDecode::worker_device(int tid) {
   int refs[3] = {-1, -1, -1};
   int slot_state[kTokSlots] = {};
   int next_slot = 0;
-  int launches_done = 0;
   int rc = VP8GPU_OK;
   ivf_worker_kit* kit = acquire_kit();
   if (!kit) rc = e->fail(VP8GPU_ERR_NOMEM, "decode_ivf: token ring allocation failed");
@@ -1381,12 +1382,21 @@ void IvfDecode::worker_device(int tid) {
   size_t head = 0, a_start[kTokSlots] = {};
   bool held[kTokSlots] = {};
   long n_takes = 0, n_wraps = 0, n_waits = 0;
-  // VP8GPU_TRACE: per chunk, timing events at "staged" (copy stream), "k_tokens may start" and "ready" (kernel stream)
+  // VP8GPU_TRACE: per chunk, timing events at "staged" (copy stream), "k_tokens may start" and "its last frame ready"
+  // (kernel stream), and %globaltimer stamps in mapped host memory: row `stamp` = "staged", then each frame's "ready"
   struct ChunkTrace {
     cudaEvent_t ev[3];
     int frames;
+    int stamp;  // -1: no stamps (more chunks than kTraceStamps)
   };
   std::vector<ChunkTrace> chunk_trace;
+  constexpr int kTraceStamps = 1024;
+  const int stamp_row = tok_chunk + 1;
+  unsigned long long* stamps = nullptr;
+  unsigned long long* stamps_dev = nullptr;
+  if (knobs.trace && (cudaHostAlloc(&stamps, sizeof(unsigned long long) * stamp_row * kTraceStamps, cudaHostAllocMapped) != cudaSuccess ||
+                      cudaHostGetDevicePointer(reinterpret_cast<void**>(&stamps_dev), stamps, 0) != cudaSuccess))
+    stamps_dev = nullptr;
   auto arena_take = [&](int si, size_t need, auto in_chunk, vp8gpu_token** out) {
     const size_t cap = arena_tokens;
     if (held[si]) {  // the slot's previous frame is done: its space is the oldest
@@ -1438,14 +1448,12 @@ void IvfDecode::worker_device(int tid) {
     uint32_t i = gop_start[g];
     while (i < gop_start[g + 1] && rc == VP8GPU_OK) {
       const uint32_t left = gop_start[g + 1] - i;
-      // slow start: the first launches of a worker are small so that its pixel work can begin
-      // after one k_tokens latency instead of after a whole chunk's parse time on top of it
-      int want = tok_chunk;
-      if (launches_done < 3 && (2 << launches_done) < want) want = 2 << launches_done;
-      launches_done++;
-      const int n = (int)left < want ? (int)left : want;
+      // one launch per GOP by default: each frame goes to the pixel kernels when its own tokens are done, so smaller
+      // first launches (2, 4, 8 frames) that let a worker's pixel work start early are not needed
+      const int n = (int)left < tok_chunk ? (int)left : tok_chunk;
       const int first_slot = next_slot;
       int staged = 0, permits_taken = 0;
+      const int stamp = stamps_dev && chunk_trace.size() < (size_t)kTraceStamps ? (int)chunk_trace.size() : -1;
       for (int c = 0; c < n && rc == VP8GPU_OK; c++) {
         const int si = (first_slot + c) % tok_slots;
         const double t0 = now();
@@ -1469,7 +1477,7 @@ void IvfDecode::worker_device(int tid) {
           return (s - first_slot + tok_slots) % tok_slots < c;
         }, &tokens);
         if (rc != VP8GPU_OK) break;
-        rc = e->token_ring_stage(kit->ring, si, p->f, kit->copy_stream, tokens);
+        rc = e->token_ring_stage(kit->ring, si, p->f, kit->copy_stream, tokens, stamp >= 0 ? stamps_dev + stamp_row * stamp + 1 + c : nullptr);
         if (rc != VP8GPU_OK) break;
         staged++;
         t_slot += t1 - t0;
@@ -1479,9 +1487,10 @@ void IvfDecode::worker_device(int tid) {
       if (rc != VP8GPU_OK) break;
       cudaStream_t ks = kit->kstream[kit->next_kstream];
       kit->next_kstream = (kit->next_kstream + 1) % kTokStreams;
+      if (stamp >= 0) vp8::launch_stamp(stamps_dev + stamp_row * stamp, kit->copy_stream);  // before k_tokens can start
       cudaEventRecord(kit->staged[first_slot], kit->copy_stream);
       cudaStreamWaitEvent(ks, kit->staged[first_slot], 0);
-      ChunkTrace ctr{{nullptr, nullptr, nullptr}, staged};
+      ChunkTrace ctr{{nullptr, nullptr, nullptr}, staged, stamp};
       if (knobs.trace) {
         for (cudaEvent_t& ev : ctr.ev) cudaEventCreate(&ev);
         cudaEventRecord(ctr.ev[0], kit->copy_stream);
@@ -1498,14 +1507,11 @@ void IvfDecode::worker_device(int tid) {
       const int until_wrap = tok_slots - first_slot;
       rc = e->token_ring_launch(kit->ring, first_slot, staged < until_wrap ? staged : until_wrap, ks);
       if (rc == VP8GPU_OK && staged > until_wrap) rc = e->token_ring_launch(kit->ring, 0, staged - until_wrap, ks);
-      if (rc == VP8GPU_OK)
-        cudaEventRecord(kit->ready[first_slot], ks);  // one event per launch: its frames become ready together
       if (knobs.trace) {
         cudaEventRecord(ctr.ev[2], ks);
         chunk_trace.push_back(ctr);
       }
-      // the permits come back when the stream gets here (also after a failed launch); queued after the
-      // `ready` events so that the host-function thread is not on the frames' critical path
+      // the permits come back when the stream gets here (also after a failed launch)
       if (permits_taken && cudaLaunchHostFunc(ks, tok_release_cb, new TokRelease{ctx, permits_taken}) != cudaSuccess) {
         std::lock_guard<std::mutex> lk(ctx->tok_mu);
         ctx->tok_permits += permits_taken;
@@ -1521,7 +1527,8 @@ void IvfDecode::worker_device(int tid) {
         job.out_off = (dst && desc.show_frame) ? items[i + c].out_off : -1;
         job.ring = kit->ring;
         job.ring_slot = si;
-        job.ready = kit->ready[first_slot];
+        job.ready_word = kit->ring->host_ready_word(si);
+        job.epoch = kit->ring->slot_epoch[si];
         job.finished = &kit->finished[si];
         rc = e->frame_alloc(&job.out);
         if (rc != VP8GPU_OK) break;
@@ -1535,7 +1542,8 @@ void IvfDecode::worker_device(int tid) {
           std::lock_guard<std::mutex> lk(mu);
           slot_state[si] = kQueued;
           job.tid = tid;
-        queues[tid].push_back(job);
+          job.gop = g;
+          queues[tid].push_back(job);
         }
         cv_disp[tid % n_disp].notify_one();
       }
@@ -1589,13 +1597,21 @@ void IvfDecode::worker_device(int tid) {
     if (knobs.trace) {
       fprintf(stderr, "decode_ivf arena: worker %d takes %ld wraps %ld waits %ld cap %zu slots %d chunk %d\n", tid, n_takes, n_wraps,
               n_waits, arena_tokens, tok_slots, tok_chunk);
-      // chunk latency: staged -> ready (what a dispatcher waits for) and k_tokens start -> ready (the kernel, residency included)
-      std::vector<float> lat, kern;
+      // chunk latency: staged -> head frame ready (what a dispatcher waits for before the GOP's next frame can go) and
+      // staged -> last frame ready, by the stamps; by the events, staged -> ready (launch done) and k_tokens start ->
+      // ready (the kernel, residency included).  An event of a stream that shares a hardware queue with busy streams
+      // can be taken late, so the two clocks need not agree.
+      std::vector<float> lat, kern, head, last;
       long frames = 0;
       for (ChunkTrace& c : chunk_trace) {
         float ms = 0;
         if (cudaEventElapsedTime(&ms, c.ev[0], c.ev[2]) == cudaSuccess) lat.push_back(ms);
         if (cudaEventElapsedTime(&ms, c.ev[1], c.ev[2]) == cudaSuccess) kern.push_back(ms);
+        if (c.stamp >= 0) {
+          const unsigned long long* row = stamps + stamp_row * c.stamp;
+          head.push_back((float)((double)(row[1] - row[0]) * 1e-6));
+          last.push_back((float)((double)(*std::max_element(row + 1, row + 1 + c.frames) - row[0]) * 1e-6));
+        }
         frames += c.frames;
         for (cudaEvent_t ev : c.ev) cudaEventDestroy(ev);
       }
@@ -1604,13 +1620,16 @@ void IvfDecode::worker_device(int tid) {
         std::sort(v.begin(), v.end());
         return (double)v[std::min(v.size() - 1, (size_t)(q * (v.size() - 1) + 0.5))];
       };
-      fprintf(stderr, "[trace] worker %d chunks: %zu (%ld frames); staged -> ready ms p10 %.2f p50 %.2f p90 %.2f max %.2f; "
-              "k_tokens start -> ready ms p50 %.2f p90 %.2f max %.2f\n", tid, chunk_trace.size(), frames, pct(lat, 0.1), pct(lat, 0.5),
-              pct(lat, 0.9), pct(lat, 1.0), pct(kern, 0.5), pct(kern, 0.9), pct(kern, 1.0));
+      fprintf(stderr, "[trace] worker %d chunks: %zu (%ld frames); staged -> head ready ms p10 %.2f p50 %.2f p90 %.2f max %.2f; "
+              "staged -> last frame ready ms p50 %.2f p90 %.2f max %.2f; events: staged -> ready ms p10 %.2f p50 %.2f p90 %.2f max %.2f; "
+              "k_tokens start -> ready ms p50 %.2f p90 %.2f max %.2f\n", tid, chunk_trace.size(), frames, pct(head, 0.1), pct(head, 0.5),
+              pct(head, 0.9), pct(head, 1.0), pct(last, 0.5), pct(last, 0.9), pct(last, 1.0), pct(lat, 0.1), pct(lat, 0.5), pct(lat, 0.9),
+              pct(lat, 1.0), pct(kern, 0.5), pct(kern, 0.9), pct(kern, 1.0));
     }
     std::lock_guard<std::mutex> lk(ctx->pool_mu);
     ctx->kit_pool.push_back(kit);
   }
+  if (stamps) cudaFreeHost(stamps);
 }
 
 // Dispatchers: dispatcher d serves the workers with tid % D == d on its own two lanes.  Queueing a
@@ -1619,6 +1638,7 @@ void IvfDecode::worker_device(int tid) {
 void IvfDecode::dispatcher(int di) {
   cudaSetDevice(e->device());
   std::vector<Pending> batch;
+  std::vector<size_t> take;
   std::vector<HostJob> hj;
   std::vector<int> dl_ids;
   std::vector<uint8_t*> dl_dst;
@@ -1638,25 +1658,24 @@ void IvfDecode::dispatcher(int di) {
     const double ti = now();
     {
       std::unique_lock<std::mutex> lk(mu);
-      // a queue's front is eligible once its tokens are in HBM (device-side token decoding)
-      // The answer is remembered: once the event of a chunk has fired, every frame of that chunk at the head of
-      // the queue is marked (a query takes the driver's lock, and this runs for every queue on every poll --
-      // hundreds of thousands of queries per second next to the workers' own CUDA calls).
-      auto eligible = [&](std::deque<Pending>& q) {
-        if (q.empty()) return false;
-        Pending& f = q.front();
-        if (!f.ready) return true;
-        if (cudaEventQuery(f.ready) != cudaSuccess) return false;
-        const cudaEvent_t fired = f.ready;
-        for (Pending& p : q) {
-          if (p.ready != fired) break;
-          p.ready = nullptr;
+      // A frame can go when it is the oldest queued frame of its GOP (consecutive frames of a GOP depend on each other,
+      // GOPs do not: a worker's next GOP advances next to the one it is finishing) and its tokens are in HBM (device-
+      // side token decoding): k_tokens has published the frame's epoch to its slot's word in mapped host memory.  A
+      // plain load, no driver call: this runs for every queue on every poll, next to the workers' own CUDA calls.
+      // A worker queues its GOPs one after the other, each in decode order, so the oldest frames of its GOPs are the
+      // ones whose GOP differs from the previous entry's.
+      auto each_eligible = [&](const std::deque<Pending>& q, auto&& fn) {
+        int prev_gop = -1;
+        for (size_t k = 0; k < q.size(); k++) {
+          const Pending& f = q[k];
+          if (f.gop == prev_gop) continue;
+          prev_gop = f.gop;
+          if (!f.ready_word || *f.ready_word == f.epoch) fn(k);
         }
-        return true;
       };
       auto ready = [&] {
         int n = 0;
-        for (int t = di; t < threads; t += n_disp) n += eligible(queues[t]);
+        for (int t = di; t < threads; t += n_disp) each_eligible(queues[t], [&](size_t) { n++; });
         return n;
       };
       auto queued = [&] {
@@ -1664,7 +1683,7 @@ void IvfDecode::dispatcher(int di) {
           if (!queues[t].empty()) return true;
         return false;
       };
-      // nothing signals the condition variable when a CUDA event fires: poll while frames wait for one
+      // nothing signals the condition variable when k_tokens publishes a frame: poll while frames wait for one
       while (!(running[di] == 0 && !queued()) && ready() == 0) {
         if (queued()) cv_disp[di].wait_for(lk, std::chrono::microseconds(100));
         else cv_disp[di].wait(lk);
@@ -1681,11 +1700,13 @@ void IvfDecode::dispatcher(int di) {
           break;
         }
       }
-      for (int t = di; t < threads; t += n_disp)
-        if (eligible(queues[t])) {
-          batch.push_back(queues[t].front());
-          queues[t].pop_front();
-        }
+      for (int t = di; t < threads; t += n_disp) {
+        std::deque<Pending>& q = queues[t];
+        take.clear();
+        each_eligible(q, [&](size_t k) { take.push_back(k); });
+        for (size_t k : take) batch.push_back(q[k]);
+        for (size_t j = take.size(); j-- > 0;) q.erase(q.begin() + (std::ptrdiff_t)take[j]);
+      }
       if (batch.empty() && running[di] == 0 && !queued()) break;
     }
     if (batch.empty()) continue;
@@ -1709,7 +1730,6 @@ void IvfDecode::dispatcher(int di) {
       if (b.ring) {
         j.ring = b.ring;
         j.ring_slot = b.ring_slot;
-        j.ready = nullptr;  // already fired (eligible() checked it)
         j.finished = b.finished;
         j.consumed = nullptr;
       }

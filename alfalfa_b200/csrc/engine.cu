@@ -590,6 +590,7 @@ TokenRing Engine::token_ring_layout(size_t max_frame_bytes, bool arena) const {
   r.bits_cap = (uint32_t)align_up(max_frame_bytes + 16, 256);
   r.split_cap = (uint32_t)n_mbs;
   r.tok_cap = token_cap_for(max_frame_bytes);
+  static_assert(sizeof(TokJob) <= 256, "a slot's TokJob area");
   size_t off = 256;  // TokJob
   r.probs_off = off;
   off += 1280;
@@ -599,6 +600,7 @@ TokenRing Engine::token_ring_layout(size_t max_frame_bytes, bool arena) const {
   off = align_up(off + r.bits_cap, 256);
   r.host_stride = off;
   r.result_off = off;
+  r.ready_off = off + 8;  // after the two result words
   off += 256;
   r.above_off = off;
   off = align_up(off + 2 * (size_t)g_.mb_cols, 256);
@@ -617,15 +619,20 @@ int Engine::token_ring_create(int nslots, size_t max_frame_bytes, TokenRing** ou
   TokenRing* r = new TokenRing(token_ring_layout(max_frame_bytes, arena_tokens > 0));
   r->nslots = nslots;
   r->slot_tokens.assign(nslots, nullptr);
+  r->slot_epoch.assign(nslots, 0);
   r->arena_cap = arena_tokens;
   if (cudaMalloc(&r->dev, r->stride * nslots) != cudaSuccess ||
       (arena_tokens && cudaMalloc(&r->arena, arena_tokens * sizeof(vp8gpu_token)) != cudaSuccess) ||
-      cudaHostAlloc(&r->host, r->host_stride * nslots, cudaHostAllocDefault) != cudaSuccess) {
+      cudaHostAlloc(&r->host, r->host_stride * nslots, cudaHostAllocDefault) != cudaSuccess ||
+      cudaHostAlloc(&r->ready_host, sizeof(uint32_t) * nslots, cudaHostAllocMapped) != cudaSuccess ||
+      cudaHostGetDevicePointer(reinterpret_cast<void**>(&r->ready_host_dev), r->ready_host, 0) != cudaSuccess) {
     token_ring_free(r);
     return fail(VP8GPU_ERR_NOMEM, "token ring allocation failed");
   }
-  // result words (tokens written, overflow flag) of slots that are never used must read as "fine"
-  CU(cudaMemset2D(r->dev + r->result_off, r->stride, 0, 8, (size_t)nslots));
+  // result words (tokens written, overflow flag) of slots that are never used must read as "fine"; ready words hold
+  // no epoch (0 is never one)
+  memset(r->ready_host, 0, sizeof(uint32_t) * nslots);
+  CU(cudaMemset2D(r->dev + r->result_off, r->stride, 0, 12, (size_t)nslots));
   *out = r;
   return VP8GPU_OK;
 }
@@ -636,10 +643,12 @@ void Engine::token_ring_free(TokenRing* r) {
   if (r->dev) cudaFree(r->dev);
   if (r->arena) cudaFree(r->arena);
   if (r->host) cudaFreeHost(r->host);
+  if (r->ready_host) cudaFreeHost(r->ready_host);
   delete r;
 }
 
-int Engine::token_ring_stage(TokenRing* r, int slot, const ParsedFrame& f, cudaStream_t s, vp8gpu_token* tokens) {
+int Engine::token_ring_stage(TokenRing* r, int slot, const ParsedFrame& f, cudaStream_t s, vp8gpu_token* tokens,
+                             unsigned long long* stamp) {
   const TokenWork& tw = f.tw;
   if (!tw.deferred) return fail(VP8GPU_ERR_LOGIC, "token_ring_stage: frame was not parsed with defer_tokens");
   if (tw.bits_len > r->bits_cap || f.desc.n_split > r->split_cap)
@@ -660,6 +669,10 @@ int Engine::token_ring_stage(TokenRing* r, int slot, const ParsedFrame& f, cudaS
   memcpy(j->part_len, tw.part_len, sizeof(j->part_len));
   j->nparts = tw.nparts;
   j->tok_cap = tokens ? token_cap_for(tw.bits_len) : r->tok_cap;
+  j->ready = reinterpret_cast<uint32_t*>(d + r->ready_off);
+  j->ready_host = r->ready_host_dev + slot;
+  j->epoch = r->slot_epoch[slot] = fresh_epoch();
+  j->stamp = stamp;
   memcpy(h + r->probs_off, tw.coef_probs, 1056);
   memcpy(h + r->bits_off, tw.bits, tw.bits_len);
   const size_t n_mbs = (size_t)g_.mb_cols * g_.mb_rows;
@@ -742,6 +755,8 @@ int Engine::submit(int lane, const HostJob* jobs, int n, cudaEvent_t consumed, c
         d.mbs = reinterpret_cast<const vp8gpu_mb*>(slot + j.ring->mbs_off);
         d.tokens = j.ring->slot_tokens[j.ring_slot];
         d.split = reinterpret_cast<const vp8gpu_split_mvs*>(slot + j.ring->split_off);
+        d.ready = j.ring->dev_ready_word(j.ring_slot);
+        d.ready_epoch = j.ring->slot_epoch[j.ring_slot];
       } else {
         d.mbs = reinterpret_cast<const vp8gpu_mb*>(st.dev + L.mbs_off[i]);
         d.tokens = reinterpret_cast<const vp8gpu_token*>(st.dev + L.tok_off[i]);
@@ -784,10 +799,7 @@ int Engine::submit(int lane, const HostJob* jobs, int n, cudaEvent_t consumed, c
   const size_t n_mbs = (size_t)g_.mb_cols * g_.mb_rows;
   for (int i = 0; i < n; i++) {
     const HostJob& j = jobs[i];
-    if (j.ring) {
-      if (j.ready) CU(cudaStreamWaitEvent(s, j.ready, 0));
-      continue;
-    }
+    if (j.ring) continue;
     CU(cudaMemcpyAsync(st.dev + L.mbs_off[i], j.mbs, n_mbs * sizeof(vp8gpu_mb), cudaMemcpyHostToDevice, s));
     if (j.desc->n_tokens)
       CU(cudaMemcpyAsync(st.dev + L.tok_off[i], j.tokens, (size_t)j.desc->n_tokens * sizeof(vp8gpu_token),

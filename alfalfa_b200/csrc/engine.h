@@ -44,13 +44,16 @@ struct DevJob {
   const void* ref_tmap[3]; // per reference: its three TMA tensor maps (Y, U, V; 128 bytes each) in HBM
   int* intra_progress;     // [mb_rows] wavefront counters, zeroed before launch
   int* lf_progress;        // [mb_rows]
+  // records and tokens written by k_tokens (a token-ring slot): its ready word, which holds ready_epoch once they are
+  // complete.  Every warp that reads them acquires it first (kernels.cu acquire_job); nullptr: the stream orders them.
+  const uint32_t* ready;
   vp8gpu_quant quant[4];
   uint8_t key_frame, sharpness, lf_enabled;
   uint8_t lf_force;        // != 0: every macroblock is filtered at this level instead of its record's
                            // (the encoder's loop-filter search, encoder.cc:460-508)
   uint32_t n_intra;        // intra-coded macroblocks in the frame
   uint32_t n_inter;
-  uint32_t pad2;
+  uint32_t ready_epoch;
 };
 
 // One frame's ENCODE job (device pointers): one wavefront pass that takes the reference encoder's
@@ -116,6 +119,13 @@ struct TokJob {
   uint32_t part_off[8], part_len[8];
   uint32_t nparts;            // 1, 2, 4 or 8
   uint32_t tok_cap;
+  // Published once the frame's records, tokens and result words are written: `epoch` (fresh for every staged frame,
+  // Engine::fresh_epoch) goes to the slot's word in HBM (release at gpu scope) and then to its word in mapped host
+  // memory (system scope), where the host polls it without a driver call.
+  uint32_t* ready;
+  uint32_t* ready_host;       // the device's address of the host word
+  uint32_t epoch;
+  unsigned long long* stamp;  // optional (VP8GPU_TRACE): %globaltimer when the frame is published
 };
 
 // Kernel launchers (kernels.cu, tokens.cu).  `stream` is a cudaStream_t passed as void* so this header
@@ -132,6 +142,7 @@ int launch_intra(const DevJob* jobs, int njobs, const Geom& g, int* ticket, uint
 int launch_loopfilter(const DevJob* jobs, int njobs, const Geom& g, int* ticket, uint32_t epoch, bool band, void* stream);
 // token jobs sit at the start of equally spaced ring slots: slot (first + i) % nslots for block i
 int launch_tokens(const uint8_t* ring, size_t stride, int first, int count, int nslots, const Geom& g, void* stream);
+int launch_stamp(unsigned long long* dst, void* stream);  // *dst = %globaltimer when the stream gets there (tracing)
 int launch_fetch_header(void* dst, const void* src_host_devptr, size_t bytes, void* stream);  // bytes % 16 == 0
 int launch_ssim(const uint8_t* a, const uint8_t* b, const Geom& g, float* d_windows, void* stream);
 int launch_enc_rd(const EncJob* jobs, int njobs, int rows, const Geom& g, int* ticket, void* stream);

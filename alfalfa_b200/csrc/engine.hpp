@@ -32,6 +32,14 @@ struct TokenRing {
   vp8gpu_token* arena = nullptr;  // tokens of the slots when not in the slots themselves
   size_t arena_cap = 0;           // in tokens
   std::vector<vp8gpu_token*> slot_tokens;  // where the tokens of each slot's current frame go
+  // per slot: the epoch k_tokens publishes when the slot's current frame is decoded (TokJob::epoch), in a word in HBM
+  // (ready_off of the slot) and in ready_host[slot], mapped pinned memory the host reads without a driver call
+  std::vector<uint32_t> slot_epoch;
+  uint32_t* ready_host = nullptr;
+  uint32_t* ready_host_dev = nullptr;  // the device's address of ready_host
+  size_t ready_off = 0;
+  const volatile uint32_t* host_ready_word(int i) const { return ready_host + i; }
+  const uint32_t* dev_ready_word(int i) const { return reinterpret_cast<const uint32_t*>(dev_slot(i) + ready_off); }
   uint8_t* dev_slot(int i) const { return dev + (size_t)i * stride; }
   uint8_t* host_slot(int i) const { return host + (size_t)i * host_stride; }
 };
@@ -47,11 +55,10 @@ struct HostJob {
   int n_intra = -1;    // -1: count them here
   int n_filtered = -1;
   cudaEvent_t consumed = nullptr;  // recorded as soon as this job's host arrays have been copied
-  // records already in HBM (token_ring_stage + token_ring_launch): nothing is copied, the stream
-  // waits for `ready` instead; `finished` (optional) is recorded after the job's kernels
+  // records already in HBM (token_ring_stage + token_ring_launch): nothing is copied, and the kernels acquire the
+  // slot's ready word before they read them; `finished` (optional) is recorded after the job's kernels
   const TokenRing* ring = nullptr;
   int ring_slot = 0;
-  cudaEvent_t ready = nullptr;
   cudaEvent_t* finished = nullptr;  // out: an event (owned by the engine) that fires after the job's kernels
 };
 
@@ -76,13 +83,14 @@ class Engine {
     for (const Frame& f : frames_) n += f.refcnt > 0;
     return n;
   }
-  // marks the hand-over messages of one wavefront launch; never 0, never repeats within 2^32 launches
-  uint32_t next_epoch(int kernel_bit = 3) {
-    if (!(ll_mask_ & kernel_bit)) return 0;
+  // never 0, never repeats within 2^32 calls: marks the hand-over messages of one wavefront launch, and the frame
+  // staged in a token-ring slot (so that a ready word left by an earlier frame never reads as this one's)
+  uint32_t fresh_epoch() {
     uint32_t e = ++epoch_;
     if (e == 0) e = ++epoch_;
     return e;
   }
+  uint32_t next_epoch(int kernel_bit = 3) { return (ll_mask_ & kernel_bit) ? fresh_epoch() : 0; }
   bool lf_band() const { return ll_mask_ & 4; }
   int frame_upload(int id, const uint8_t* y, size_t ys, const uint8_t* u, const uint8_t* v, size_t cs);
   int frame_download(int id, uint8_t* y, size_t ys, uint8_t* u, uint8_t* v, size_t cs);
@@ -113,7 +121,9 @@ class Engine {
   void token_ring_free(TokenRing* r);
   // queue on `s` the upload of one frame parsed with defer_tokens (records + partitions); a ring with an arena
   // takes the frame's token area (`tokens`, token_cap_for(f.tw.bits_len) tokens) from the caller
-  int token_ring_stage(TokenRing* r, int slot, const ParsedFrame& f, cudaStream_t s, vp8gpu_token* tokens = nullptr);
+  // (`stamp`, optional: where k_tokens writes %globaltimer when the frame is ready)
+  int token_ring_stage(TokenRing* r, int slot, const ParsedFrame& f, cudaStream_t s, vp8gpu_token* tokens = nullptr,
+                       unsigned long long* stamp = nullptr);
   // one k_tokens launch over `count` consecutive slots (wrapping around the ring)
   int token_ring_launch(TokenRing* r, int first, int count, cudaStream_t s);
   // queue on `s` the reset of a slot's result words; k_tokens only ever sets the overflow flag, so it stays set for

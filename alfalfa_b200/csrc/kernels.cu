@@ -521,12 +521,33 @@ __device__ __forceinline__ void add_residuals(uint8_t* pix, const int16_t* coef,
   __syncwarp();
 }
 
+// Before a warp reads a job's records, tokens or split vectors that k_tokens wrote on another stream: one acquire of
+// the slot's ready word (tokens.cu publish_ready).  It reads the epoch that k_tokens released, and so synchronizes
+// with it: the host submitted the job only after it saw the epoch in the slot's host word, k_tokens wrote the device
+// word before the host word (system-scope fence between them), and the slot is staged again only after this frame's
+// pixel kernels have finished, so the device word holds the epoch from before this launch until after it.
+__device__ __forceinline__ void acquire_job(const DevJob& J, int lane) {
+  const uint32_t* w = J.ready;
+  if (!w) return;  // records ordered by the stream (host uploads, or k_tokens on the same stream)
+  if (lane == 0) {
+#ifndef VP8GPU_SIMT_EMUL
+    uint32_t v;
+    asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(w) : "memory");
+#else
+    // tests/simt: the word must already hold the job's epoch (streams run in order there)
+    if (__atomic_load_n(w, __ATOMIC_ACQUIRE) != J.ready_epoch) abort();
+#endif
+  }
+  __syncwarp();  // the other lanes' later loads are ordered after lane 0's acquire through this barrier
+}
+
 __global__ void __launch_bounds__(INTER_WARPS * 32, 10) k_inter(const DevJob* __restrict__ jobs, Geom g) {
   __shared__ InterSmem s_all[INTER_WARPS];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const DevJob& J = jobs[blockIdx.y];
   const int mbi = blockIdx.x * INTER_WARPS + warp;
   if (mbi >= g.mb_cols * g.mb_rows) return;
+  acquire_job(J, lane);
   const MbFields f = load_mb(J.mbs + mbi);
   if (f.ref == VP8GPU_REF_CURRENT) return;  // intra macroblocks belong to k_intra
   const int row = mbi / g.mb_cols, col = mbi - row * g.mb_cols;
@@ -839,6 +860,7 @@ __global__ void __launch_bounds__(32 * WF_WARPS, 24) k_intra(const DevJob* __res
   if (row >= g.mb_rows) return;
   const DevJob& J = jobs[job];
   if (J.n_intra == 0) return;
+  acquire_job(J, lane);
   const int cols = g.mb_cols;
   const vp8gpu_mb* row_mbs = J.mbs + (size_t)row * cols;
 
@@ -1126,6 +1148,7 @@ __global__ void __launch_bounds__(32 * WF_WARPS, 16) k_loopfilter(const DevJob* 
   if (row >= g.mb_rows) return;
   const DevJob& J = jobs[job];
   if (!J.lf_enabled) return;
+  acquire_job(J, lane);
   const int cols = g.mb_cols;
   const vp8gpu_mb* row_mbs = J.mbs + (size_t)row * cols;
 
@@ -1318,6 +1341,7 @@ __global__ void __launch_bounds__(32 * LF_BAND, 32 / LF_BAND) k_loopfilter_band(
   if (row >= g.mb_rows) return;
   const DevJob& J = jobs[job];
   if (!J.lf_enabled) return;
+  acquire_job(J, lane);
   const int cols = g.mb_cols;
   const vp8gpu_mb* row_mbs = J.mbs + (size_t)row * cols;
   Row* const S = s_rows + warp;

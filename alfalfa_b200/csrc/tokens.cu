@@ -26,6 +26,27 @@ namespace vp8 {
 namespace {
 
 constexpr int kMaxCols = 1024;  // 16383 px / 16
+
+// The frame's records, tokens and result words are written (by this thread): publish its epoch.  The release at gpu
+// scope orders those writes before the device word, which the pixel kernels acquire (kernels.cu acquire_job); the
+// system-scope fence orders the device word before the host word, so that a host that has seen the host word
+// launches pixel kernels that find the device word set.
+__device__ __forceinline__ void publish_ready(const TokJob& J) {
+#ifndef VP8GPU_SIMT_EMUL
+  asm volatile("st.release.gpu.global.u32 [%0], %1;" ::"l"(J.ready), "r"(J.epoch) : "memory");
+  asm volatile("fence.acq_rel.sys;" ::: "memory");
+  asm volatile("st.relaxed.sys.global.u32 [%0], %1;" ::"l"(J.ready_host), "r"(J.epoch) : "memory");
+  if (J.stamp) {
+    unsigned long long t;
+    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+    *J.stamp = t;
+  }
+#else
+  __atomic_store_n(J.ready, J.epoch, __ATOMIC_RELEASE);
+  __atomic_store_n(J.ready_host, J.epoch, __ATOMIC_RELEASE);
+  if (J.stamp) *J.stamp = 1;
+#endif
+}
 // jobs live at the start of equally spaced slots of a ring (engine.hpp TokenRing); one warp per frame,
 // kTokWarps frames per CTA (measured: one-warp CTAs spread over the SMs best; VP8GPU_TOK_WARPS=8 packs them)
 template <int kTokWarps>
@@ -44,6 +65,7 @@ __global__ void __launch_bounds__(32 * kTokWarps) k_tokens(const uint8_t* ring, 
   __syncwarp();
   if (lane != 0) return;
   tok::decode_frame_tokens(J, g, probs, above_nz);
+  publish_ready(J);
 }
 
 // lock-step variant: one LANE per frame, 32 frames per warp (tokens_core.cuh decode_frame_tokens_lockstep).
@@ -76,9 +98,25 @@ __global__ void __launch_bounds__(32) k_tokens_lockstep(const uint8_t* ring, siz
   __syncwarp();
   if (!J) return;
   tok::decode_frame_tokens_lockstep<32>(*J, g, T, P + lane, above + lane);
+  publish_ready(*J);
+}
+
+__global__ void k_stamp(unsigned long long* dst) {
+#ifndef VP8GPU_SIMT_EMUL
+  unsigned long long t;
+  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+  *dst = t;
+#else
+  *dst = 0;
+#endif
 }
 
 }  // namespace
+
+int launch_stamp(unsigned long long* dst, void* stream) {
+  VP8_LAUNCH(k_stamp, 1, 1, 0, static_cast<cudaStream_t>(stream))(dst);
+  return (int)cudaGetLastError();
+}
 
 int launch_tokens(const uint8_t* ring, size_t stride, int first, int count, int nslots, const Geom& g, void* stream) {
   if (g.mb_cols > kMaxCols) return (int)cudaErrorInvalidValue;

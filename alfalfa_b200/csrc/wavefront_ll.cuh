@@ -136,6 +136,7 @@ __global__ void __launch_bounds__(32 * WF_WARPS, 18) k_intra_ll(const DevJob* __
   if (row >= g.mb_rows) return;
   const DevJob& J = jobs[job];
   if (J.n_intra == 0) return;
+  acquire_job(J, lane);
   const int cols = g.mb_cols;
   const vp8gpu_mb* row_mbs = J.mbs + (size_t)row * cols;
 
@@ -402,6 +403,7 @@ __global__ void __launch_bounds__(32 * WF_WARPS, 14) k_loopfilter_ll(const DevJo
   if (row >= g.mb_rows) return;
   const DevJob& J = jobs[job];
   if (!J.lf_enabled) return;
+  acquire_job(J, lane);
   const int cols = g.mb_cols;
   const vp8gpu_mb* row_mbs = J.mbs + (size_t)row * cols;
   const bool last_row = row == g.mb_rows - 1;

@@ -1,7 +1,7 @@
 #!/usr/bin/env python3
 """GPU-box tool: sweep the host-side knobs of vp8gpu_decode_ivf on the bench workload (output left on the device)
 and print Mpix/s, the host time accounting and -- with --trace (VP8GPU_TRACE=1) -- the per-batch device times of every
-dispatcher and, per worker, the distribution of its chunks' latency from "staged" to "ready" (k_tokens).
+dispatcher and, per worker, the distribution of its chunks' latency from "staged" to "head frame ready" and to "ready" (k_tokens).
 The bench shape: --configs 64:4:5 --streams 258.
 usage: tools/e2e_probe.py [--configs "threads:dispatchers:nice,..."] [--steps N] [--trace]"""
 import argparse

@@ -13,6 +13,9 @@ with the product's bitstream writer like tools/make_edge_stream.py.  Seeded and 
   sizemix_WxH      GOPs of 1, 2, 3, 31, 32, 33, 95, 96, 97 and 200 frames (chunk boundaries, slot-ring wrap, GOPs longer
                    than the ring) mixing runs of near-largest dense frames, mid-size frames, all-skip inter frames of a
                    few bytes and hidden ALTREF frames, so that the token arena of every worker wraps and waits
+  largestlast_WxH  GOPs of 30 frames whose last frame is by far the largest (its tokens are decoded last in a k_tokens
+  largestfirst_WxH launch), or whose key frame is (decoded last, and the rest of its launch ready long before)
+                   (order_names(): a catalogue of their own, checked against the host-token path, not stored answers)
 
 usage: python tools/make_pipeline_stream.py NAME OUT.ivf        (NAME one of names())
 """
@@ -200,10 +203,33 @@ def make_sizemix(w, h, seed):
     return F.ivf(w, h, chunks), nparts
 
 
+# ---------------------------------------------------------------- largest frame last / first
+ORDER_SIZES = [(176, 144)]
+ORDER_GOPS, ORDER_GOP_LEN = 4, 30
+
+
+def make_order(w, h, seed, largest_last):
+    """GOPs of small frames (skip and half-coded at +-1) with one frame at +-2114 everywhere: the last or the key frame"""
+    L, capi = _lib()
+    rng = np.random.default_rng(seed)
+    saved = np.zeros(1056, dtype=np.uint8)
+    chunks = []
+    for g in range(ORDER_GOPS):
+        for i in range(ORDER_GOP_LEN):
+            big = i == (ORDER_GOP_LEN - 1 if largest_last else 0)
+            kind = "key" if i == 0 else ("mixed" if big else ("skip" if (g + i) % 3 == 0 else "half"))
+            chunks.append(_frame(L, capi, rng, w, h, saved, i == 0, (g + i) % 4, _pick(kind), value=MAX_COEF if big else 1))
+    return F.ivf(w, h, chunks), [1 << (g + i) % 4 for g in range(ORDER_GOPS) for i in range(ORDER_GOP_LEN)]
+
+
 # ---------------------------------------------------------------- catalogue
 def names():
     return (["density_%dx%d_p%d" % (w, h, p) for w, h in DENSITY_SIZES for p in DENSITY_PARTS] + [DENSITY_1080] +
             ["densemix_%dx%d" % s for s in DENSEMIX_SIZES] + [DENSEGOP] + ["sizemix_%dx%d" % s for s in SIZEMIX_SIZES])
+
+
+def order_names():
+    return ["largest%s_%dx%d" % (o, w, h) for o in ("last", "first") for w, h in ORDER_SIZES]
 
 
 def make(name):
@@ -226,12 +252,14 @@ def make_with_partitions(name):
         return make_densegop(w, h, 750 + w)
     if parts[0] == "sizemix":
         return make_sizemix(w, h, 800 + w)
+    if parts[0] in ("largestlast", "largestfirst"):
+        return make_order(w, h, 900 + w + (parts[0] == "largestfirst"), parts[0] == "largestlast")
     raise KeyError(name)
 
 
 if __name__ == "__main__":
     if len(sys.argv) != 3:
-        sys.exit(__doc__ + "\nnames: " + " ".join(names()))
+        sys.exit(__doc__ + "\nnames: " + " ".join(names() + order_names()))
     data = make(sys.argv[1])
     open(sys.argv[2], "wb").write(data)
     print("%s: %d bytes" % (sys.argv[2], len(data)))
